@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the Ctrl-Adapter denoising hot path on B200 (contract: see the task brief / DESIGN.md section 6).
+"""Benchmark of the Ctrl-Adapter denoising hot path on H100 (see DESIGN.md section 6).
 
   python bench.py --gpus N --steps K --warmup W            ours: CUDA path (this repo's kernels)
+  python bench.py ... --dump-outputs DIR                   also write what the last timed step computed (DIR/*.npy)
   python bench.py --impl reference --gpus N ...            reference arm: the oracle restatement of the reference's
                                                            PyTorch path on the host CPU cores (diffusers is not
                                                            installable here, so the reference itself cannot run)
@@ -89,6 +90,8 @@ def parse():
                    help="do not time the oracle (restated reference) as eager bf16-autocast PyTorch on this GPU")
     p.add_argument("--skip-profile", action="store_true", help="skip the per-kernel CUDA-event profile (roofline block)")
     p.add_argument("--cpu-budget-s", type=float, default=45.0, help="wall-clock budget of the cpu_baseline leg")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write the last step's outputs (latents, next model input) as float32 .npy")
     return p.parse_args()
 
 
@@ -244,7 +247,7 @@ def build_oracle_stepper(workload, inp, device, dtype, batch):
 
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -287,7 +290,8 @@ def measured_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- a ceiling, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -479,6 +483,16 @@ def workload_name(workload, batch, res):
                      f"batch {batch} per GPU"}[workload] + f" (CFG: {n} frame-samples), one pipeline-loop iteration per step"
 
 
+def dump_outputs(out_dir, arrays):
+    """What the timed path hands its caller after its last step -- the updated latents and, on one GPU, the scaled
+    model input of the next step -- as float32 .npy (a few MB for every workload at its default batch)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 # ----------------------------------------------------------------------------------------------------
 _RESULT_FD = None
 
@@ -548,13 +562,17 @@ def main():
         stepfn((a.warmup + i) % nsteps)
     if dist:  # the single collective of the job: gather every rank's final latents (C1 in SURVEY.md)
         from ctrl_adapter_b200.distributed import gather_latents
-        gathered = gather_latents(loop.latents, loop.latents.shape[0] * world)  # noqa: F841
+        gathered = gather_latents(loop.latents, loop.latents.shape[0] * world)
     ev1.record()
     torch.cuda.synchronize()
     if dist:
         dist.barrier()
     ms_total = ev0.elapsed_time(ev1)
     clocks = sampler.stop()
+    if a.dump_outputs and rank == 0:
+        # across GPUs the caller receives the gathered latents; the next model input stays a per-rank shard
+        dump_outputs(a.dump_outputs, {"latents": gathered} if dist else
+                     {"latents": loop.latents, "model_in": loop.model_in})
     if dist:
         tt = torch.tensor([ms_total], device=dev)
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -607,44 +625,26 @@ def main():
         loop.step(0)
         ops.PROFILER.stop()
         fam = ops.PROFILER.summary()
-        try:
-            os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-            json.dump(ops.PROFILER.launches_table(80),
-                      open(os.path.join(ROOT, "gpurun_out", f"launch_table_{a.workload}.json"), "w"), indent=0)
-        except Exception:
-            pass
         tot = sum(v["ms"] for v in fam.values())
         families = {k: {"launches": v["launches"], "ms": round(v["ms"], 3), "share": round(v["ms"] / tot, 4),
                         "tflops": round(v["flops"] / (v["ms"] * 1e9), 2) if v["ms"] > 0 and v["flops"] else None,
                         "gbs": round(v["bytes"] / (v["ms"] * 1e6), 1) if v["ms"] > 0 and v["bytes"] else None}
                     for k, v in sorted(fam.items(), key=lambda kv: -kv[1]["ms"])}
         top = max(fam.items(), key=lambda kv: kv[1]["ms"])
-        # DRAM bytes per launch of the dominant kernel: ncu dram__bytes_{read,write}.sum over every launch of one step
-        # (profiles/r?_traffic_<workload>.json, made by scripts/launch_share.py from the committed launch list)
-        traffic = None
-        for rnd in ("r2", "r1"):
-            try:
-                tj = json.load(open(os.path.join(ROOT, "profiles", f"{rnd}_traffic_{a.workload}.json")))
-                kn = {"gemm": "gemm_conv_kernel", "attention": "attention_kernel"}.get(top[0])
-                if kn in tj:
-                    traffic = round(tj[kn]["dram_bytes_per_launch"], 0)
-                    break
-            except Exception:
-                continue
         if top[0] in ("gemm", "attention"):
             ach = top[1]["flops"] / (top[1]["ms"] * 1e9)
             peak = peaks["bf16_tflops_sustained"]
-            roofline = {"kernel": {"gemm": "gemm_conv_kernel (tcgen05 multi-tap GEMM / implicit conv)",
-                                   "attention": "attention_kernel (tcgen05 flash attention)"}[top[0]],
+            roofline = {"kernel": {"gemm": "gemm_conv_kernel (wgmma multi-tap GEMM / implicit conv)",
+                                   "attention": "attention_kernel (wgmma flash attention)"}[top[0]],
                         "bound": "tensor", "achieved": round(ach, 2), "peak": peak, "unit": "TFLOP/s",
-                        "frac": round(ach / peak, 4), "traffic": traffic,
+                        "frac": round(ach / peak, 4),
                         "how": f"sum of algorithmic FLOPs of the {top[1]['launches']} launches of one step / sum of their "
                                f"CUDA-event durations ({top[1]['ms']:.1f} ms = {100 * top[1]['ms'] / tot:.0f}% of the step); "
                                f"peak = bf16_tflops_sustained, {peak_src}"}
         else:
             ach = top[1]["bytes"] / (top[1]["ms"] * 1e6)
             roofline = {"kernel": top[0], "bound": "hbm", "achieved": round(ach, 1), "peak": peaks["hbm_gbs"],
-                        "unit": "GB/s", "frac": round(ach / peaks["hbm_gbs"], 4), "traffic": None,
+                        "unit": "GB/s", "frac": round(ach / peaks["hbm_gbs"], 4),
                         "how": f"algorithmic bytes / CUDA-event time of one step; peak {peak_src}"}
 
     # ---- "reference single-GPU eager PyTorch" (BASELINE.md section 3, the north-star denominator): oracle modules, bf16
@@ -697,7 +697,7 @@ def main():
             "data": "synthetic",
             "config": {"workload": workload_name(a.workload, batch, a.res), "baseline_config": w["base"],
                        "parallelism": f"batch-sharded dp{world}", "cuda_graph": use_graph,
-                       "l2": "per-step working set (multi-GB bf16 weights + multi-GB activations) exceeds the 126 MB L2; "
+                       "l2": "per-step working set (multi-GB bf16 weights + multi-GB activations) exceeds the 50 MB L2; "
                              "no explicit flush",
                        "algorithmic_tflop_per_step": round(step_tflop, 1),
                        "step_tflops_achieved": round(step_tflop / (ms_step / 1000.0), 1),

@@ -109,7 +109,7 @@ def load():
         raise CtrlAdapterB200Error(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(there is no CPU / PyTorch fallback for the hot path)")
-    # CA_B200_LIB: developer override (e.g. the -DCA_TRACE build made by scripts/gemm_trace.py)
+    # CA_B200_LIB: developer override (another build of the library, e.g. -DCA_NO_PDL)
     lib = C.CDLL(os.environ.get("CA_B200_LIB", LIB_PATH))
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -1,4 +1,4 @@
-"""B200 host mirror of the reference adapter modules.
+"""H100 host mirror of the reference adapter modules.
 
 ``ControlNetAdapter`` / ``AdapterSpatioTemporal`` / ``ControlNetRouter`` keep the reference's constructor kwargs,
 forward signatures, return structures and state-dict keys (/root/reference/model/ctrl_adapter.py:17-44,171-224;
@@ -6,7 +6,7 @@ model/adapter_spatial_temporal.py:11-37,175-292; model/ctrl_router.py:49-58,85-1
 pipelines can use them unchanged.  Tensors cross the boundary as logical NCHW; physically everything is channels-last
 (``torch.channels_last`` outputs, zero-copy when the producer is another module of this package).
 
-All arithmetic runs in the sm_100a kernels (see layers.py / ops.py); there is no PyTorch fallback.
+All arithmetic runs in the sm_90a kernels (see layers.py / ops.py); there is no PyTorch fallback.
 """
 from __future__ import annotations
 

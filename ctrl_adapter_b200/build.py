@@ -1,4 +1,4 @@
-"""In-tree build of libctrl_adapter_b200.so: nvcc cross-compiles every .cu for sm_100a (works without a GPU)."""
+"""In-tree build of libctrl_adapter_b200.so: nvcc cross-compiles every .cu for sm_90a (works without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -10,10 +10,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libctrl_adapter_b200.so")
-SOURCES = ["gemm_conv.cu", "gemm_conv_bn64.cu", "gemm_conv_bn128.cu", "gemm_conv_bn160.cu", "gemm_conv_bn256.cu", "gemm_conv_wide.cu",
+SOURCES = ["gemm_conv.cu", "gemm_conv_bn64.cu", "gemm_conv_bn128.cu", "gemm_conv_bn160.cu", "gemm_conv_bn256.cu",
            "attention.cu", "temporal_attention.cu", "norm.cu", "elementwise.cu", "capi.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _newer(target: str, deps) -> bool:
@@ -46,7 +46,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
             list(ex.map(run, jobs))
     if jobs or force or not _newer(LIB, objs):
-        run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", LIB] + objs)
+        run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-cudart", "static", "-o", LIB] + objs)
     return LIB
 
 

@@ -1,4 +1,4 @@
-"""B200 host mirror of the frozen SD1.5 ControlNet (/root/reference/controlnet/controlnet.py:107-881) and of
+"""H100 host mirror of the frozen SD1.5 ControlNet (/root/reference/controlnet/controlnet.py:107-881) and of
 ``MultiControlNetModel`` (/root/reference/controlnet/multicontrolnet.py:45-99).
 
 Same constructor kwargs (default SD1.5 topology), forward signature (including the reference's ``skip_conv_in`` /
@@ -34,7 +34,7 @@ class ControlNetConditioningEmbedding(nn.Module):
 
     # the 8- / 16- / 32-channel stride-1 convolutions at full image resolution run with 8 / 4 / 2 adjacent pixels folded
     # into the channel axis (layers.Conv2d.forward_folded) instead of padding every tap to 64 channels; GPU-verified in
-    # round 2 (profiles/r2_parity.md, group `fold`; -1.3 ms / SDXL step).  CA_FOLD_SMALL_CONV=0 restores the padded form.
+    # round 2 (checked by the GPU test group `fold`).  CA_FOLD_SMALL_CONV=0 restores the padded form.
     def forward(self, cond_nhwc8):
         fold = os.environ.get("CA_FOLD_SMALL_CONV", "1") != "0"
         conv = (lambda m, x, **kw: m.forward_folded(x, **kw)) if fold else (lambda m, x, **kw: m(x, **kw))

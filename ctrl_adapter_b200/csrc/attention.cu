@@ -1,69 +1,32 @@
 // Fused softmax(Q K^T * scale) V for the spatial self / cross attention of the adapter, the ControlNet and the
-// UNets.  tcgen05 MMAs with TMEM accumulators, TMA-fed 128B-swizzled shared memory, online softmax in registers.
+// UNets: wgmma tensor-core MMAs, TMA-fed 128B-swizzled shared memory, online softmax in registers.
 //
-// One CTA = 128 query rows of one (batch, head) and one 64-wide slice of the value head dim; 128 + 128 * NS threads
-// (NS = number of softmax warpgroups = column splits of a score row, 1 or 2):
-//   warpgroup 0: warp 0 = TMA producer (Q once, then K and V tiles of 128 keys through SEPARATE 2-stage rings:
-//                a K slot is free as soon as its QK^T retired, so K runs two tiles ahead of the softmax),
-//                warp 1 = MMA issuer + TMEM allocator.  S = Q K^T (M128 N128, K = 64*DQ) into TMEM cols [0,128);
-//                O += P V (M128 N64 K128, V consumed MN-major) ACCUMULATED in TMEM cols [128,192).  Warps 2-3 idle.
-//   warpgroups 1..NS: softmax.  NS = 1 (the default): one thread per query row.  NS = 2 (CA_ATTN_SPLIT=2, evaluated in
-//                round 2 and NOT adopted -- same time, profiles/r2_ncu_attn4k_split2.md): two threads per row -- warp w
-//                and warp w + 4 own the same 32 TMEM lanes and split the 128 key columns of the tile 64 / 64; the row
-//                max is combined through a 1 KB shared-memory exchange and a 64-thread named barrier per warp pair,
-//                the row sum and the output columns stay split until the item's epilogue.
-//                Per KV tile the scores of the row (half) are read from TMEM ONCE
-//                (tcgen05.ld, one wait) and the S buffer is released immediately so the next tile's QK^T overlaps
-//                this tile's softmax.  The running max is "lazy": O (in TMEM) and the row sum are rescaled only when a
-//                row's max grew by more than 2^8 since the max in use (exact: softmax is shift invariant and exp2
-//                arguments stay <= 8), so the common path never touches O.
-// The softmax warps are the bottleneck (the tensor pipe idles ~70%), so their instruction stream is what is optimised:
-//   * packed fp32x2 FFMA2 / FADD2 for the scale-and-shift and the row sum (half-rate instructions -- 2 clk of the FMA
-//     pipe each, scripts/ubench/pipes.cu -- so they save issue slots, not pipe time);
-//   * the exp schedule is THROTTLED (template TH): without it ptxas starts every long FMA-pipe chain first and leaves ~50
-//     MUFU.EX2 back to back at the end of a tile, during which the warp issues nothing else; routing each group's
-//     shift constant through fma(row_sum_of_group_g-2, 0, shift) -- numerically a no-op, but a true dependency -- keeps
-//     the MUFUs within two groups of their FMA work (783 -> 815 TFLOP/s at 16k x 16k, d = 64);
-//   * MUFU.EX2 (16 / clk / SM) is the scarcest pipe: a compile-time share of the exponentials (kPolyOf8 pairs out of
-//     8) is evaluated on the FMA pipe instead -- Cody-Waite split, cubic minimax 2^f on [-0.5, 0.5] (7.5e-5 relative,
-//     1/26 of a bf16 half-ulp of P), exponent spliced in with an integer add;
-//   * setmaxnreg moves registers from warpgroup 0 to the softmax warpgroup(s) (NS = 1: 208 each, NS = 2: 96 each;
-//     warpgroup 0 keeps 48 -- with fewer the MMA issuer spills its descriptors and every tcgen05.mma issue costs hundreds
-//     of cycles) so the scores of a row (half) stay in registers without spills while two CTAs still share an SM;
-//   * the producer / MMA warps back off with nanosleep while blocked so their polling does not steal issue slots.
-// With head dim 64 the CTA uses 101 KB smem (two Q buffers, two K and two V tiles) / 256 TMEM columns, so two CTAs share
-// an SM and one CTA's softmax overlaps the other's MMAs.  Head dims 128/192 (the zero-padded ControlNet heads) use DQ = 2/3 (one CTA per SM).
-#include <cstdlib>
-#include <type_traits>
-
+// One CTA = 128 query rows of one (batch, head) and one 64-wide slice of the value head dim; 384 threads:
+//   warpgroup 0, one thread: TMA producer (Q once, then K and V tiles of 128 keys through a 2-stage ring)
+//   warpgroups 1, 2        : 64 query rows each.  Per KV tile: S = Q K^T (m64n128, K = 64 * DQ, both operands K-major
+//                            in shared memory) into registers; online softmax (exp2, running max and row sum in fp32);
+//                            P is rounded to bf16 and fed from registers as the A operand of O += P V (m64n64, V read
+//                            MN-major from shared memory).  The ring slot is released once both wgmma have retired.
+// Epilogue: O / l, one bf16 rounding, 4-byte stores.  Head dims 128 / 192 (the zero-padded ControlNet heads) use
+// DQ = 2 / 3 chunks of 64 for Q K^T.
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace ca {
 
-static constexpr int kThrottleDefault = 4;  // round-2 A/B (profiles/r2_experiments.md): 783 -> 815 TFLOP/s at 16k x 16k
-static constexpr int kSplitDefault = 1;  // softmax warpgroups per CTA (column halves of a score row) for head dim 64
-static constexpr int kPolyDefault = 2;  // pairs out of every 8 whose exp2 runs on the FMA pipe instead of MUFU
 static constexpr int kTileQ = 128;
 static constexpr int kTileKV = 128;
+static constexpr int kAttnThreads = 384;
 static constexpr uint32_t kChunkBytes = 128 * 64 * 2;  // one [128 rows x 64 cols] bf16 swizzle tile = 16 KB
-static constexpr float kRescaleThreshold = 8.0f;       // log2 units
 
 template <int DQ>
 struct AttnCfg {
   static constexpr int kStages = 2;
   static constexpr uint32_t kQBytes = DQ * kChunkBytes;
-  // Q is double buffered (round 2) where shared memory allows: with a single buffer the load of the next item's Q tile
-  // could only start when this item's last QK^T had retired, and its ~2 us of HBM latency was exposed once per work item
-  // -- which is most of an item when there is ONE KV tile (the 77-key cross attention ran at 0.3 of its HBM bound)
-  static constexpr int kQStages = (DQ <= 2) ? 2 : 1;
-  static constexpr uint32_t kPBytes = 4096;  // row max / row sum exchange of the NS = 2 variant (P itself lives in TMEM)
   static constexpr uint32_t kStageBytes = (DQ + 1) * kChunkBytes;  // K chunks + one V slice
-  // data + 1024: the slack serves both the 1024-byte alignment of the swizzled tiles and the mbarriers.
-  // For DQ == 1 this is 115712 B, i.e. exactly two CTAs per SM: 2 x (115712 + 1024 reserved) = 233472 = 228 KB.
-  static constexpr uint32_t kDataBytes = kQStages * kQBytes + kPBytes + kStages * kStageBytes;
-  static constexpr uint32_t kSmemBytes = kDataBytes + 1024;
-  static constexpr uint32_t kTmemCols = 256;
+  static constexpr uint32_t kDataBytes = kQBytes + kStages * kStageBytes;
+  static constexpr uint32_t kSmemBytes = kDataBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -72,828 +35,197 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// 2^x for a pair on the FMA / ALU pipes only.  x <= 8 by construction; clamped below so the exponent splice cannot wrap
-// (anything under 2^-100 is irrelevant next to a row sum >= 2^-8).
-__device__ __forceinline__ void exp2_poly_x2(float x0, float x1, float& p0, float& p1) {
-  const uint64_t x = pack_f32x2(fmaxf(x0, -100.0f), fmaxf(x1, -100.0f));
-  const uint64_t t = add_f32x2(x, pack_f32x2(12582912.0f, 12582912.0f));          // round(x) lands in the mantissa
-  const uint64_t r = add_f32x2(t, pack_f32x2(-12582912.0f, -12582912.0f));         // round(x) as a float
-  const uint64_t f = fma_f32x2(r, pack_f32x2(-1.0f, -1.0f), x);                     // x - round(x) in [-0.5, 0.5]
-  uint64_t p = fma_f32x2(pack_f32x2(0.0551716685f, 0.0551716685f), f, pack_f32x2(0.2426111251f, 0.2426111251f));
-  p = fma_f32x2(p, f, pack_f32x2(0.6932609677f, 0.6932609677f));
-  p = fma_f32x2(p, f, pack_f32x2(0.9999280572f, 0.9999280572f));
-  float t0, t1, q0, q1;
-  unpack_f32x2(t, t0, t1);
-  unpack_f32x2(p, q0, q1);
-  p0 = __int_as_float(__float_as_int(q0) + (__float_as_int(t0) << 23));
-  p1 = __int_as_float(__float_as_int(q1) + (__float_as_int(t1) << 23));
-}
-template <int POLY>
-__host__ __device__ constexpr bool pair_uses_poly(int pair) {  // POLY of every 8 pairs, evenly spread
-  return ((pair % 8 + 1) * POLY) / 8 != ((pair % 8) * POLY) / 8;
-}
-
-template <int R>
-__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R>
-__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
-
-// blocked for a long time by design (producer on a free K/V slot, MMA issuer on the softmax): poll politely
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity, unsigned ns) {
-  int polls = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if (++polls > 8 && ns > 0) __nanosleep(ns);  // short waits never sleep
-  }
-}
-
-// 64-thread named barrier of the warp pair (w, w + 4) that shares TMEM lane quarter q; immediate ids so that the kernel
-// reserves 5 hardware barriers, not all 16 (two CTAs share an SM)
-__device__ __forceinline__ void pair_bar_sync(int q) {
-  switch (q) {
-    case 0: asm volatile("bar.sync 1, 64;" ::: "memory"); break;
-    case 1: asm volatile("bar.sync 2, 64;" ::: "memory"); break;
-    case 2: asm volatile("bar.sync 3, 64;" ::: "memory"); break;
-    default: asm volatile("bar.sync 4, 64;" ::: "memory"); break;
-  }
-}
-
-template <int DQ, int POLY, int NS, int TH>
-__global__ void __launch_bounds__(128 + 128 * NS, (DQ == 1) ? 2 : 1)
+template <int DQ>
+__global__ void __launch_bounds__(kAttnThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
   using Cfg = AttnCfg<DQ>;
   CA_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
-  uint8_t* smem = smem_raw + pad;
-  if (pad + Cfg::kDataBytes + 192 > Cfg::kSmemBytes) __trap();  // barriers would not fit behind the tiles
-  constexpr int kCols = kTileKV / NS;     // score columns per softmax thread
-  constexpr int kChunks = kCols / 32;     // 32-column TMEM loads per thread and tile
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* smem_q = smem;
-  uint8_t* smem_p = smem + Cfg::kQStages * Cfg::kQBytes;
-  [[maybe_unused]] float* xch_max = reinterpret_cast<float*>(smem_p);          // [2 tile parities][2 halves][128 rows]
-  [[maybe_unused]] float* xch_sum = reinterpret_cast<float*>(smem_p) + 512;    // [2 halves][128 rows]
-  uint8_t* smem_kv = smem_p + Cfg::kPBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_kv + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* q_full = bars + 14;   // [2]
-  uint64_t* k_full = bars + 1;    // [2]
-  uint64_t* k_empty = bars + 3;   // [2]
-  uint64_t* v_full = bars + 10;   // [2]
-  uint64_t* v_empty = bars + 12;  // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* s_empty = bars + 6;
-  uint64_t* p_full = bars + 7;
-  uint64_t* o_full = bars + 8;
-  uint64_t* q_empty = bars + 16;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
+  uint8_t* smem_kv = smem + Cfg::kQBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kDataBytes);
+  uint64_t* q_full = bars;
+  uint64_t* full = bars + 1;   // [kStages]
+  uint64_t* empty = bars + 3;  // [kStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int q0 = blockIdx.x * kTileQ;
+  const int h = blockIdx.y / p.v_slices;
+  const int vs = blockIdx.y % p.v_slices;
+  const int b = blockIdx.z;
   const int dpad = 64 * p.v_slices;  // padded head dim (elements) in the Q/K/V channel layout
   const int nkv = (p.lk + kTileKV - 1) / kTileKV;
-  // persistent CTA: work item w = (v slice, batch*head, query tile), query tile fastest so that the CTAs running at the
-  // same time share K/V through L2.  Each role walks the same item sequence; barrier parities come from per-CTA counters
-  // (it = items done, g = KV tiles done) so the pipelines run straight across item boundaries: the next item's Q / K
-  // loads and first QK^T overlap this item's last softmax, PV and output write.
-  const int nqt = (p.lq + kTileQ - 1) / kTileQ;
-  const int total_items = nqt * p.batch * p.heads * p.v_slices;
-  auto decode = [&](int w, int& q0, int& b, int& h, int& vs) {
-    q0 = (w % nqt) * kTileQ;
-    const int bh = (w / nqt) % (p.batch * p.heads);
-    vs = w / (nqt * p.batch * p.heads);
-    b = bh / p.heads;
-    h = bh % p.heads;
-  };
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&q_full[s], 1);
-      mbar_init(&q_empty[s], 1);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // one arrive per consumer warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 4 * NS);
-    mbar_init(p_full, 4 * NS);
-    mbar_init(o_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base;
-  const uint32_t tmem_o = tmem_base + 128;
-  CA_PDL_WAIT();  // prologue (barriers, TMEM) done: from here on global memory of the previous kernel is consumed
-  const uint32_t tmem_p = tmem_base + 192;  // bf16 P (A operand of the PV TS MMA), two keys per 32-bit cell, 64 columns
-
-  if (warp < 4) {
-    if constexpr (DQ == 1) setmaxnreg_dec<48>();
-  }
-  if (warp == 0) {
-    if (lane == 0) {
-      TR_DECL(tr_kv_empty);
-      uint32_t it = 0, g = 0;  // items / KV tiles issued so far by this CTA
-      TR_EVT_DECL(0);
-      int q0, b, h, vs;
-      auto load_k = [&](int j, uint32_t gk, int kvb) {
-        const int st = gk & 1;
-        uint8_t* dst = smem_kv + st * Cfg::kStageBytes;
-        TR_WAIT(tr_kv_empty, mbar_wait_backoff(&k_empty[st], ((gk >> 1) & 1) ^ 1, p.backoff_ns));
-        mbar_arrive_expect_tx(&k_full[st], DQ * kChunkBytes);
-        for (int c = 0; c < DQ; ++c)
-          tma_load_3d(dst + c * kChunkBytes, &tmap_k, &k_full[st], h * dpad + c * 64, j * kTileKV, kvb);
-      };
-      for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++it) {
-        decode(w, q0, b, h, vs);
-        const int kvb = b / p.kv_batch_div;
-        const int qs = it % Cfg::kQStages;
-        // every QK^T of the item that used this Q buffer (one or two items ago) has retired
-        mbar_wait_backoff(&q_empty[qs], ((it / Cfg::kQStages) & 1) ^ 1, p.backoff_ns);
-        TR_EVT(1);
-        mbar_arrive_expect_tx(&q_full[qs], Cfg::kQBytes);
-        for (int c = 0; c < DQ; ++c)
-          tma_load_3d(smem_q + qs * Cfg::kQBytes + c * kChunkBytes, &tmap_q, &q_full[qs], h * dpad + c * 64, q0, b);
-        load_k(0, g, kvb);
-        TR_EVT(2);
-        for (int j = 0; j < nkv; ++j, ++g) {
-          // K(j+1) first: its slot frees when QK^T(j-1) retires, which precedes PV(j-2) (the condition for V(j))
-          if (j + 1 < nkv) load_k(j + 1, g + 1, kvb);
-          const int st = g & 1;
-          TR_WAIT(tr_kv_empty, mbar_wait_backoff(&v_empty[st], ((g >> 1) & 1) ^ 1, p.backoff_ns));
-          mbar_arrive_expect_tx(&v_full[st], kChunkBytes);
-          tma_load_3d(smem_kv + st * Cfg::kStageBytes + DQ * kChunkBytes, &tmap_v, &v_full[st], h * dpad + vs * 64,
-                      j * kTileKV, kvb);
-          TR_EVT(3);
-        }
-      }
-      TR_PUT(9, tr_kv_empty);
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64, 0, 1);  // B (= V tile) is MN-major
-      const uint32_t q_base = smem_u32(smem_q);
-      TR_DECL(tr_kv_full);
-      TR_DECL(tr_s_empty);
-      TR_DECL(tr_p_full);
-      TR_DECL(tr_q_full);
-      TR_EVT_DECL(96);
-      [[maybe_unused]] const long long tr_start = TR_NOW();
-      const int my_items = (total_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                           static_cast<int>(gridDim.x);
-      const uint32_t total_tiles = static_cast<uint32_t>(my_items) * nkv;
-      // QK^T of global tile gq (tile jq of item itq); waits for that item's Q when jq == 0
-      auto issue_qk = [&](uint32_t gq, int jq, uint32_t itq) {
-        const int st = gq & 1;
-        const int qs = itq % Cfg::kQStages;
-        const uint32_t q_addr = q_base + qs * Cfg::kQBytes;
-        if (jq == 0) TR_WAIT(tr_q_full, mbar_wait_backoff(&q_full[qs], (itq / Cfg::kQStages) & 1, p.backoff_ns));
-        TR_EVT(10);
-        TR_WAIT(tr_kv_full, mbar_wait(&k_full[st], (gq >> 1) & 1));
-        TR_WAIT(tr_s_empty, mbar_wait(s_empty, (gq & 1) ^ 1));  // softmax has read S of the previous tile
-        TR_EVT(11);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(smem_kv + st * Cfg::kStageBytes);
-#pragma unroll
-        for (int c = 0; c < DQ; ++c) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = umma_smem_desc_sw128(q_addr + c * kChunkBytes + k * 32, 16, 1024);
-            const uint64_t db = umma_smem_desc_sw128(k_addr + c * kChunkBytes + k * 32, 16, 1024);
-            umma_bf16_ss(tmem_s, da, db, idesc_s, (c | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(s_full);
-        umma_commit(&k_empty[st]);               // K slot reusable once this QK^T has retired
-        if (jq == nkv - 1) umma_commit(&q_empty[qs]);  // ... and so is this Q buffer after the item's last QK^T
-        TR_EVT(12);
-      };
-      if (total_tiles > 0) issue_qk(0, 0, 0);
-      uint32_t g = 0;
-      for (int it = 0; it < my_items; ++it) {
-        for (int j = 0; j < nkv; ++j, ++g) {
-          // look-ahead QK^T of the same item goes first; the first QK^T of the NEXT item waits for that item's Q, so it
-          // is issued after this item's last PV instead of delaying it (and with it the output write)
-          if (j + 1 < nkv) issue_qk(g + 1, j + 1, it);
-          const int st = g & 1;
-          TR_WAIT(tr_kv_full, mbar_wait(&v_full[st], (g >> 1) & 1));
-          TR_EVT(13);
-          TR_WAIT(tr_p_full, mbar_wait_backoff(p_full, g & 1, p.backoff_ns));  // P staged and (if it was needed) O rescaled
-          TR_EVT(14);
-          tc_fence_after();
-          const uint32_t v_addr = smem_u32(smem_kv + st * Cfg::kStageBytes + DQ * kChunkBytes);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint64_t db = umma_smem_desc_sw128(v_addr + k * 2048, 8192, 1024);
-            umma_bf16_ts(tmem_o, tmem_p + k * 8, db, idesc_o, (j | k) != 0 ? 1u : 0u);  // 16 keys = 8 TMEM cells
-          }
-          umma_commit(o_full);
-          umma_commit(&v_empty[st]);
-          TR_EVT(15);
-          if (j + 1 == nkv && g + 1 < total_tiles) issue_qk(g + 1, 0, it + 1);
-        }
-      }
-      TR_PUT(5, tr_kv_full);
-      TR_PUT(6, tr_s_empty);
-      TR_PUT(7, tr_p_full);
-      TR_PUT(10, tr_q_full);
-      TR_PUT(8, TR_NOW() - tr_start);
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax / output: NS threads per query row =====================
-    if constexpr (DQ == 1) setmaxnreg_inc<(NS == 1) ? 208 : 96>();
-    // the two persistent CTAs of an SM start together; offset one of them by about half a KV tile so their MUFU-heavy
-    // exp phases interleave instead of colliding (whichever way the hardware pairs block ids onto SMs)
-    if (p.stagger_ns > 0 && gridDim.x > 148 && (((blockIdx.x / 148) ^ blockIdx.x) & 1)) __nanosleep(p.stagger_ns);
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int hf = (warp - 4) >> 2;         // column half (0 for NS == 1)
-    const int r = q * 32 + lane;
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    const uint32_t s_col = static_cast<uint32_t>(hf * kCols);             // first score column of this thread
-    const uint32_t p_cell = static_cast<uint32_t>(hf * (kCols / 2));      // first packed-P cell (two keys per cell)
-    constexpr int kOCols = 64 / NS;                                        // output columns this thread rescales / writes
-    const uint32_t o_col = static_cast<uint32_t>(hf * kOCols);
-    const float sl2 = p.scale_log2;
-    float m_used = -INFINITY;  // the max (raw score units) the accumulated P / O / l are expressed against
-    float l_run = 0.f;         // row sum over this thread's columns
-    TR_DECL(tr_s_full);
-    TR_DECL(tr_o_full);
-    TR_DECL(tr_ld);
-    TR_DECL(tr_resc);
-    TR_DECL(tr_epi_o);
-    TR_EVT_DECL(192);
-    [[maybe_unused]] const bool tr_me = (warp == 4 && lane == 0);
-    [[maybe_unused]] const long long tr_start = TR_NOW();
-
-    auto tile_step = [&](auto mask_tag, int j, uint32_t g, int kv_valid) {
-      constexpr bool MASK = decltype(mask_tag)::value;
-      TR_WAIT(tr_s_full, mbar_wait(s_full, g & 1));
-      if (tr_me) TR_EVT(20);
-      tc_fence_after();
-      // partial last KV tile: only the 32-column chunks that hold a valid key are processed (the P columns
-      // of the others are written as zeros); inside the boundary chunk invalid scores become -inf, so the
-      // code below is the same as for a full tile
-      const int my_valid = MASK ? max(0, min(kCols, kv_valid - static_cast<int>(s_col))) : kCols;
-      const int nch = MASK ? (my_valid + 31) >> 5 : kChunks;
-      // ---- pass 1 over the scores (TMEM -> registers, transient): row max ----
-      // The scores are read from tensor memory TWICE (max pass, exp pass) instead of being held in registers across
-      // both: a tcgen05.ld of 32 columns costs a few issue cycles, while 64-128 live score registers per thread are what
-      // limits the number of softmax warps an SM can hold (the register file, not the MUFU pipe, is the scarce resource).
-      // NS == 1 has the registers (208) to keep the whole row: ONE read, and the S buffer is released right away so the
-      // next tile's QK^T overlaps all of this tile's softmax.  NS == 2 (96 registers) re-reads the scores in pass 2.
-      constexpr bool kTwoPass = (NS == 2);
-      float m_tile;
-      uint32_t sv[kChunks][32];
-      {
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c) tmem_ld_32x32(tmem_s + lane_sel + s_col + c * 32, sv[c]);
-        TR_WAIT(tr_ld, tmem_ld_wait());
-        if constexpr (!kTwoPass) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(s_empty);  // S is in registers: the next QK^T may overwrite the TMEM buffer
-        }
-        float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c) {
-          if (MASK && c >= nch) continue;
-          const int lim = my_valid - c * 32;
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float a0 = (!MASK || i < lim) ? __uint_as_float(sv[c][i]) : -INFINITY;
-            const float a1 = (!MASK || i + 1 < lim) ? __uint_as_float(sv[c][i + 1]) : -INFINITY;
-            mx0 = fmaxf(mx0, a0);
-            mx1 = fmaxf(mx1, a1);
-          }
-        }
-        m_tile = fmaxf(mx0, mx1);
-      }
-      if (tr_me) TR_EVT(21);
-      if constexpr (NS == 2) {
-        // combine with the thread that owns the other 64 columns of this row (warp +-4, same lane): buffers alternate
-        // with the tile parity, so a thread running ahead never overwrites a value its partner has not read yet
-        float* slot = xch_max + (g & 1) * 256;
-        slot[hf * 128 + r] = m_tile;
-        pair_bar_sync(q);
-        m_tile = fmaxf(m_tile, slot[(hf ^ 1) * 128 + r]);
-      }
-      // ---- lazy rescale: only when this row's max exceeds the max in use by more than 2^8 ----
-      bool waited_o = false;
-      if (j == 0) {
-        m_used = m_tile;
-      } else {
-        const bool need = (m_tile - m_used) * sl2 > kRescaleThreshold;
-        if (__any_sync(0xffffffffu, need)) {  // both halves of a row take the same decision (same m_tile, m_used)
-#ifdef CA_TRACE
-          ++tr_resc;
-#endif
-          mbar_wait(o_full, (g - 1) & 1);  // PV of tile j-1 has landed in O
-          tc_fence_after();
-          waited_o = true;
-          const float alpha = need ? fast_exp2((m_used - m_tile) * sl2) : 1.0f;
-          if (need) m_used = m_tile;
-          l_run *= alpha;
-#pragma unroll
-          for (int c = 0; c < kOCols / 32; ++c) {
-            uint32_t ov[32];
-            tmem_ld_32x32(tmem_o + lane_sel + o_col + c * 32, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st_32x32(tmem_o + lane_sel + o_col + c * 32, ov);
-          }
-          tmem_st_wait();
-        }
-      }
-      // ---- pass 2: p = exp2(s*sl2 - m_used*sl2) (<= 2^8), row sum, bf16 P, 32 columns at a time ----
-      const float mneg = -m_used * sl2;
-      const uint64_t sl2_2 = pack_f32x2(sl2, sl2), mneg_2 = pack_f32x2(mneg, mneg);
-      // Row sum in three rotating accumulators.  TH > 0 ("throttle"): the scale-and-shift constant of every group of TH
-      // column pairs is routed through  fma(rs_of_group_g-2, 0, mneg)  -- numerically mneg, but a TRUE dependency on the
-      // exponentials of two groups earlier.  ptxas otherwise starts all the long FMA-pipe chains first and leaves ~50
-      // MUFU.EX2 back to back at the end of the tile (profiles/r2_ncu_attn4k_base.md: 22 % of the softmax time), during
-      // which this warp can issue nothing else; the dependency keeps the MUFUs within two groups of their FMA work.
-      uint64_t rs3[3] = {pack_f32x2(0.f, 0.f), pack_f32x2(0.f, 0.f), pack_f32x2(0.f, 0.f)};
-      const uint64_t zero2 = pack_f32x2(0.f, 0.f);
-      // packed bf16 P overwrites the already consumed scores in place (sv[c][0..15]) and is kept there until the previous
-      // PV has released the P buffer in tensor memory
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        if (MASK && c >= nch) {
-          if (kTwoPass && c == kChunks - 1) {  // the S buffer is released by the last chunk's turn even when it is empty
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(s_empty);
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i) sv[c][i] = 0u;  // P = 0 for keys that do not exist
-        } else {
-          uint32_t (&sc)[32] = sv[c];
-          if constexpr (kTwoPass) {
-            tmem_ld_32x32(tmem_s + lane_sel + s_col + c * 32, sc);
-            tmem_ld_wait();
-            if (c == kChunks - 1) {  // every score of the tile has been read for the last time: the next QK^T may start
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(s_empty);
-            }
-          }
-          const int lim = my_valid - c * 32;  // valid columns of this chunk (warp-uniform; >= 32 except in the boundary chunk)
-          uint64_t mn = mneg_2;
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            constexpr int kGroup = TH > 0 ? TH : 16;
-            const int pair = c * 16 + (i >> 1);
-            const int grp = pair / kGroup;
-            if (TH > 0 && pair % kGroup == 0 && grp >= 2) mn = fma_f32x2(rs3[(grp + 1) % 3], zero2, mneg_2);
-            const float s0 = (!MASK || i < lim) ? __uint_as_float(sc[i]) : -INFINITY;
-            const float s1 = (!MASK || i + 1 < lim) ? __uint_as_float(sc[i + 1]) : -INFINITY;
-            const uint64_t x = fma_f32x2(pack_f32x2(s0, s1), sl2_2, mn);
-            float x0, x1, p0, p1;
-            unpack_f32x2(x, x0, x1);
-            if (pair_uses_poly<POLY>(i >> 1)) {
-              exp2_poly_x2(x0, x1, p0, p1);  // -inf (masked) is clamped: 2^-100, invisible next to a row sum >= 1
-            } else {
-              p0 = fast_exp2(x0);
-              p1 = fast_exp2(x1);
-            }
-            rs3[grp % 3] = add_f32x2(rs3[grp % 3], pack_f32x2(p0, p1));
-            sc[i >> 1] = pack_bf16x2(p0, p1);
-          }
-        }
-      }
-      {
-        float rs0, rs1;
-        unpack_f32x2(add_f32x2(add_f32x2(rs3[0], rs3[1]), rs3[2]), rs0, rs1);
-        l_run += rs0 + rs1;
-      }
-      if (tr_me) TR_EVT(22);
-      // P of tile j-1 must have been consumed by its PV MMA before it is overwritten (waiting here, after the
-      // exponentials, the PV issued at the end of the previous tile has long retired)
-      if (j > 0 && !waited_o) {
-        TR_WAIT(tr_o_full, mbar_wait(o_full, (g - 1) & 1));
-        tc_fence_after();
-      }
-      // P goes to tensor memory (the PV MMA reads its A operand from there): no shared-memory stores, no proxy fence
-#pragma unroll
-      for (int c = 0; c < kChunks; ++c)
-        tmem_st_32x16(tmem_p + lane_sel + p_cell + c * 16, *reinterpret_cast<const uint32_t(*)[16]>(&sv[c][0]));
-      tmem_st_wait();
-      tc_fence_before();         // orders the tcgen05.st (P, and O of a rescale) before the MMA that follows the barrier
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      if (tr_me) TR_EVT(23);
-    };
-    uint32_t g = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x) {
-      int q0, b, h, vs;
-      decode(w, q0, b, h, vs);
-      m_used = -INFINITY;
-      l_run = 0.f;
-      for (int j = 0; j < nkv; ++j, ++g) {
-        const int kv_valid = min(kTileKV, p.lk - j * kTileKV);
-        if (kv_valid == kTileKV) tile_step(std::false_type{}, j, g, kv_valid);
-        else tile_step(std::true_type{}, j, g, kv_valid);
-      }
-      // epilogue: O / l (the next item's first QK^T and its loads are already in flight)
-      float l_row = l_run;
-      if constexpr (NS == 2) {
-        // the row sum is split like the columns; single buffer: at least one max exchange (a barrier of this warp pair)
-        // separates two epilogues, so the partner has read the previous item's value before it is overwritten
-        xch_sum[hf * 128 + r] = l_run;
-        pair_bar_sync(q);
-        l_row += xch_sum[(hf ^ 1) * 128 + r];
-      }
-      TR_WAIT(tr_epi_o, mbar_wait(o_full, (g - 1) & 1));
-      if (tr_me) TR_EVT(24);
-      tc_fence_after();
-      const float inv_l = 1.0f / l_row;
-      const int row = q0 + r;
-      __nv_bfloat16* orow = p.out + static_cast<long long>(b) * p.out_batch_stride +
-                            static_cast<long long>(row) * p.out_row_stride + h * dpad + vs * 64 + o_col;
-#pragma unroll
-      for (int c = 0; c < kOCols / 32; ++c) {
-        uint32_t ov[32];
-        tmem_ld_32x32(tmem_o + lane_sel + o_col + c * 32, ov);
-        tmem_ld_wait();
-        if (row < p.lq) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(ov[u * 8 + e]) * inv_l;
-            *reinterpret_cast<uint4*>(orow + c * 32 + u * 8) = make_uint4(
-                pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-          }
-        }
-      }
-      if (tr_me) TR_EVT(25);
-      tc_fence_before();  // O reads ordered before the p_full arrive that lets the next item's first PV overwrite O
-    }
-    if (warp == 4 && lane == 0) {
-      TR_PUT(0, TR_NOW() - tr_start);
-      TR_PUT(1, tr_s_full);
-      TR_PUT(2, tr_o_full);
-      TR_PUT(3, tr_resc);
-      TR_PUT(4, tr_ld);
-      TR_PUT(11, tr_epi_o);
-    }
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Short-KV variant: Lk <= 80 (the 77-token text cross attention of the ControlNet / SDXL UNet), head dim 64.
-// There is ONE KV tile per work item, so the tile loop that hides the PV latency and the output write in the general
-// kernel does not exist: there the four softmax warps wait for PV(i), then write item i out, and only then start on
-// item i + 1 (profiles/r2_ncu_attn77.md: 156 TFLOP/s, nothing busy).  Here
-//   * S is M128 x N80 and P 40 packed cells, which leaves tensor memory for TWO output accumulators
-//     (columns: O0 [0,64)  O1 [64,128)  S [128,208)  P [208,248)),
-//   * the MMA warp issues QK^T(i+1) BEFORE PV(i) (S is free as soon as the softmax has it in registers), and
-//   * the softmax warps write item i - 1 out AFTER they have staged P(i): PV(i) and QK^T(i+1) run under that epilogue.
-// No running max / rescale: one tile is the whole row.  Same producer, barriers and Q / K / V rings as above.
-// ---------------------------------------------------------------------------------------------------------------
-static constexpr int kShortKV = 80;
-
-template <int POLY>
-__global__ void __launch_bounds__(256, 2)
-attention_short_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                       const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
-  using Cfg = AttnCfg<1>;
-  CA_PDL_TRIGGER();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
-  uint8_t* smem = smem_raw + pad;
-  if (pad + Cfg::kDataBytes + 192 > Cfg::kSmemBytes) __trap();
-  uint8_t* smem_q = smem;
-  uint8_t* smem_kv = smem + Cfg::kQStages * Cfg::kQBytes + Cfg::kPBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_kv + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* q_full = bars + 14;   // [2]
-  uint64_t* k_full = bars + 1;    // [2]
-  uint64_t* k_empty = bars + 3;   // [2]
-  uint64_t* v_full = bars + 10;   // [2]
-  uint64_t* v_empty = bars + 12;  // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* s_empty = bars + 6;
-  uint64_t* p_full = bars + 7;
-  uint64_t* o_full = bars + 8;
-  uint64_t* q_empty = bars + 16;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int dpad = 64 * p.v_slices;
-  const int nqt = (p.lq + kTileQ - 1) / kTileQ;
-  const int total_items = nqt * p.batch * p.heads * p.v_slices;
-  auto decode = [&](int w, int& q0, int& b, int& h, int& vs) {
-    q0 = (w % nqt) * kTileQ;
-    const int bh = (w / nqt) % (p.batch * p.heads);
-    vs = w / (nqt * p.batch * p.heads);
-    b = bh / p.heads;
-    h = bh % p.heads;
-  };
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&q_full[s], 1);
-      mbar_init(&q_empty[s], 1);
-      mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 4);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_o = tmem_base;         // two accumulators of 64 columns
-  const uint32_t tmem_s = tmem_base + 128;   // 80 fp32 score columns
-  const uint32_t tmem_p = tmem_base + 208;   // 40 cells of packed bf16 P
   CA_PDL_WAIT();
 
-  if (warp < 4) setmaxnreg_dec<48>();
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++it) {
-        int q0, b, h, vs;
-        decode(w, q0, b, h, vs);
-        const int kvb = b / p.kv_batch_div;
-        const int st = it & 1;
-        const uint32_t free_parity = ((it >> 1) & 1) ^ 1;
-        uint8_t* kv = smem_kv + st * Cfg::kStageBytes;
-        mbar_wait_backoff(&q_empty[st], free_parity, p.backoff_ns);
-        mbar_arrive_expect_tx(&q_full[st], Cfg::kQBytes);
-        tma_load_3d(smem_q + st * Cfg::kQBytes, &tmap_q, &q_full[st], h * dpad, q0, b);
-        mbar_wait_backoff(&k_empty[st], free_parity, p.backoff_ns);
-        mbar_arrive_expect_tx(&k_full[st], kChunkBytes);
-        tma_load_3d(kv, &tmap_k, &k_full[st], h * dpad, 0, kvb);
-        mbar_wait_backoff(&v_empty[st], free_parity, p.backoff_ns);
-        mbar_arrive_expect_tx(&v_full[st], kChunkBytes);
-        tma_load_3d(kv + kChunkBytes, &tmap_v, &v_full[st], h * dpad + vs * 64, 0, kvb);
+  if (warp < 4) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      const int kvb = b / p.kv_batch_div;
+      mbar_arrive_expect_tx(q_full, Cfg::kQBytes);
+      for (int c = 0; c < DQ; ++c) tma_load_3d(smem_q + c * kChunkBytes, &tmap_q, q_full, h * dpad + c * 64, q0, b);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int j = 0; j < nkv; ++j) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        uint8_t* dst = smem_kv + stage * Cfg::kStageBytes;
+        mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
+        for (int c = 0; c < DQ; ++c)
+          tma_load_3d(dst + c * kChunkBytes, &tmap_k, &full[stage], h * dpad + c * 64, j * kTileKV, kvb);
+        tma_load_3d(dst + DQ * kChunkBytes, &tmap_v, &full[stage], h * dpad + vs * 64, j * kTileKV, kvb);
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, kShortKV, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64, 0, 1);  // B (= V tile) is MN-major
-      const uint32_t q_base = smem_u32(smem_q);
-      const int my_items = (total_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                           static_cast<int>(gridDim.x);
-      auto issue_qk = [&](uint32_t i) {
-        const int st = i & 1;
-        const uint32_t ph = (i >> 1) & 1;
-        mbar_wait_backoff(&q_full[st], ph, p.backoff_ns);
-        mbar_wait(&k_full[st], ph);
-        mbar_wait(s_empty, (i & 1) ^ 1);  // the softmax holds S of the previous item in registers
-        tc_fence_after();
-        const uint32_t q_addr = q_base + st * Cfg::kQBytes;
-        const uint32_t k_addr = smem_u32(smem_kv + st * Cfg::kStageBytes);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = umma_smem_desc_sw128(q_addr + k * 32, 16, 1024);
-          const uint64_t db = umma_smem_desc_sw128(k_addr + k * 32, 16, 1024);
-          umma_bf16_ss(tmem_s, da, db, idesc_s, k != 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        umma_commit(&k_empty[st]);
-        umma_commit(&q_empty[st]);
-      };
-      if (my_items > 0) issue_qk(0);
-      for (int i = 0; i < my_items; ++i) {
-        if (i + 1 < my_items) issue_qk(i + 1);
-        const int st = i & 1;
-        mbar_wait(&v_full[st], (i >> 1) & 1);
-        mbar_wait_backoff(p_full, i & 1, p.backoff_ns);  // P(i) staged; O[i & 1] was written out two items ago
-        tc_fence_after();
-        const uint32_t v_addr = smem_u32(smem_kv + st * Cfg::kStageBytes + kChunkBytes);
-#pragma unroll
-        for (int k = 0; k < kShortKV / 16; ++k) {
-          const uint64_t db = umma_smem_desc_sw128(v_addr + k * 2048, 8192, 1024);
-          umma_bf16_ts(tmem_o + (i & 1) * 64, tmem_p + k * 8, db, idesc_o, k != 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(&v_empty[st]);
-      }
-    }
-  } else if (warp >= 4) {
-    setmaxnreg_inc<208>();
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    const float sl2 = p.scale_log2;
-    const int lk = p.lk;
-    // writes work item w out: O[buf] / l (PV of that item has completed: the caller waited for o_full)
-    auto write_out = [&](int w, float l, uint32_t buf) {
-      int q0, b, h, vs;
-      decode(w, q0, b, h, vs);
-      const float inv_l = 1.0f / l;
-      const int row = q0 + r;
-      __nv_bfloat16* orow = p.out + static_cast<long long>(b) * p.out_batch_stride +
-                            static_cast<long long>(row) * p.out_row_stride + h * dpad + vs * 64;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t ov[32];
-        tmem_ld_32x32(tmem_o + lane_sel + buf * 64 + c * 32, ov);
-        tmem_ld_wait();
-        if (row < p.lq) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(ov[u * 8 + e]) * inv_l;
-            *reinterpret_cast<uint4*>(orow + c * 32 + u * 8) = make_uint4(
-                pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-          }
-        }
-      }
-      tc_fence_before();  // the O reads are ordered before the next p_full arrive (after which PV may overwrite O[buf])
-    };
-    int w_prev = -1;
-    float l_prev = 1.f;
-    uint32_t i = 0;
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++i) {
-      mbar_wait(s_full, i & 1);
-      tc_fence_after();
-      uint32_t sv[kShortKV];
-      tmem_ld_32x32(tmem_s + lane_sel, *reinterpret_cast<uint32_t(*)[32]>(&sv[0]));
-      tmem_ld_32x32(tmem_s + lane_sel + 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[32]));
-      tmem_ld_32x16(tmem_s + lane_sel + 64, *reinterpret_cast<uint32_t(*)[16]>(&sv[64]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty);  // S is in registers: QK^T of the next item may overwrite it
-      float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < kShortKV; c += 2) {
-        mx0 = fmaxf(mx0, c < lk ? __uint_as_float(sv[c]) : -INFINITY);
-        mx1 = fmaxf(mx1, c + 1 < lk ? __uint_as_float(sv[c + 1]) : -INFINITY);
-      }
-      const float mneg = -fmaxf(mx0, mx1) * sl2;
-      const uint64_t sl2_2 = pack_f32x2(sl2, sl2), mneg_2 = pack_f32x2(mneg, mneg);
-      uint64_t rs[2] = {pack_f32x2(0.f, 0.f), pack_f32x2(0.f, 0.f)};
-#pragma unroll
-      for (int c = 0; c < kShortKV; c += 2) {
-        const float s0 = c < lk ? __uint_as_float(sv[c]) : -INFINITY;  // keys that do not exist: p = 0
-        const float s1 = c + 1 < lk ? __uint_as_float(sv[c + 1]) : -INFINITY;
-        const uint64_t x = fma_f32x2(pack_f32x2(s0, s1), sl2_2, mneg_2);
-        float x0, x1, p0, p1;
-        unpack_f32x2(x, x0, x1);
-        if (pair_uses_poly<POLY>(c >> 1)) {
-          exp2_poly_x2(x0, x1, p0, p1);
-        } else {
-          p0 = fast_exp2(x0);
-          p1 = fast_exp2(x1);
-        }
-        rs[(c >> 1) & 1] = add_f32x2(rs[(c >> 1) & 1], pack_f32x2(p0, p1));
-        sv[c >> 1] = pack_bf16x2(p0, p1);  // in place: cell c / 2 was consumed at least one iteration ago
-      }
-      float r0, r1;
-      unpack_f32x2(add_f32x2(rs[0], rs[1]), r0, r1);
-      const float l = r0 + r1;
-      if (i > 0) {  // PV(i-1) has read P(i-1) and completed O[(i-1) & 1]
-        mbar_wait(o_full, (i - 1) & 1);
-        tc_fence_after();
-      }
-      tmem_st_32x16(tmem_p + lane_sel, *reinterpret_cast<const uint32_t(*)[16]>(&sv[0]));
-      tmem_st_32x16(tmem_p + lane_sel + 16, *reinterpret_cast<const uint32_t(*)[16]>(&sv[16]));
-      tmem_st_32x8(tmem_p + lane_sel + 32, *reinterpret_cast<const uint32_t(*)[8]>(&sv[32]));
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      if (i > 0) write_out(w_prev, l_prev, (i - 1) & 1);  // under PV(i) and QK^T(i+1)
-      w_prev = w;
-      l_prev = l;
-    }
-    if (w_prev >= 0) {
-      mbar_wait(o_full, (i - 1) & 1);
-      tc_fence_after();
-      write_out(w_prev, l_prev, (i - 1) & 1);
-    }
+    return;
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+  // ===================== consumers =====================
+  setmaxnreg_inc<232>();
+  const int cw = (warp >> 2) - 1;  // query rows [64 cw, 64 cw + 64) of the tile
+  const int wq = warp & 3;
+  const int tig = lane & 3;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};
+  float l_run[2] = {0.f, 0.f};
+  const uint32_t q_addr = smem_u32(smem_q) + cw * 64 * 128;
+  mbar_wait(q_full, 0);
+
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int j = 0; j < nkv; ++j) {
+    mbar_wait(&full[stage], phase);
+    const uint32_t kv_addr = smem_u32(smem_kv + stage * Cfg::kStageBytes);
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < DQ; ++c) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        Wgmma<128>::ss(s, gmma_desc_sw128(q_addr + c * kChunkBytes + k * 32, 16, 1024),
+                       gmma_desc_sw128(kv_addr + c * kChunkBytes + k * 32, 16, 1024), (c | k) != 0 ? 1 : 0);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // ---- online softmax: thread holds rows (r, r + 8) x key columns 8 jj + 2 tig + {0, 1} ----
+    const int kv_valid = min(kTileKV, p.lk - j * kTileKV);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = 8 * jj + 2 * tig + (e & 1);
+        float x = s[4 * jj + e] * p.scale_log2;
+        if (col >= kv_valid) x = -INFINITY;
+        s[4 * jj + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+    float corr[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      const float m_new = fmaxf(m_run[hh], mx[hh]);
+      corr[hh] = fast_exp2(m_run[hh] - m_new);  // 0 on the first tile (m_run = -inf)
+      m_run[hh] = m_new;
+      l_run[hh] *= corr[hh];
+    }
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float pv = fast_exp2(s[4 * jj + e] - m_run[e >> 1]);
+        s[4 * jj + e] = pv;
+        l_run[e >> 1] += pv;
+      }
+    }
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= corr[(i >> 1) & 1];
+
+    // ---- O += P V ----
+    const uint32_t v_addr = kv_addr + DQ * kChunkBytes;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) Wgmma<64>::rs_bt(o, pa[kk], gmma_desc_sw128(v_addr + kk * 2048, 8192, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (lane == 0) mbar_arrive(&empty[stage]);
+    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+  }
+
+  // ---- epilogue: O / l ----
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float l = l_run[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.0f / l;
+    const int row = q0 + cw * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+    if (row >= p.lq) continue;
+    __nv_bfloat16* orow = p.out + static_cast<long long>(b) * p.out_batch_stride +
+                          static_cast<long long>(row) * p.out_row_stride + h * dpad + vs * 64;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * tig) =
+          pack_bf16x2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
+    }
   }
 }
 
-template <int POLY>
-static cudaError_t launch_short(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p,
-                                cudaStream_t stream) {
-  using Cfg = AttnCfg<1>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_short_kernel<POLY>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(Cfg::kSmemBytes));
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_short_kernel<POLY>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                             cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  static int resident = 0;
-  if (resident == 0) {
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaError_t e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess || sms < 1) return e != cudaSuccess ? e : cudaErrorInvalidConfiguration;
-    resident = sms * 2;
-  }
-  const long long items = static_cast<long long>((p.lq + kTileQ - 1) / kTileQ) * p.batch * p.heads * p.v_slices;
-  if (items <= 0 || items > 0x7fffffffLL) return cudaErrorInvalidValue;
-  const int grid = static_cast<int>(items < resident ? items : resident);
-  auto kern = attention_short_kernel<POLY>;
-  CA_KERNEL_LAUNCH(kern, grid, 256, Cfg::kSmemBytes, stream, q, k, v, p);
-  return cudaGetLastError();
-}
-
-template <int DQ, int POLY, int NS, int TH = 0>
+template <int DQ>
 static cudaError_t launch_dq(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p,
                              cudaStream_t stream) {
   using Cfg = AttnCfg<DQ>;
   static bool attr_set = false;
+  auto kern = attention_kernel<DQ>;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel<DQ, POLY, NS, TH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(Cfg::kSmemBytes));
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_kernel<DQ, POLY, NS, TH>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                             cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  static int resident = 0;  // CTAs the device holds at once: two per SM for head dim 64 (smem), else one
-  if (resident == 0) {
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaError_t e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess || sms < 1) return e != cudaSuccess ? e : cudaErrorInvalidConfiguration;
-    resident = sms * (DQ == 1 ? 2 : 1);
-  }
-  const long long items = static_cast<long long>((p.lq + kTileQ - 1) / kTileQ) * p.batch * p.heads * p.v_slices;
-  if (items <= 0 || items > 0x7fffffffLL) return cudaErrorInvalidValue;
-  // developer knobs: CA_ATTN_GRID=items launches one CTA per work item (hardware block scheduler, dynamic balance)
-  static const bool per_item = getenv("CA_ATTN_GRID") && getenv("CA_ATTN_GRID")[0] == 'i';
-  const int grid = static_cast<int>((items < resident || per_item) ? items : resident);
-  auto kern = attention_kernel<DQ, POLY, NS, TH>;
-  CA_KERNEL_LAUNCH(kern, grid, 128 + 128 * NS, Cfg::kSmemBytes, stream, q, k, v, p);
+  const dim3 grid((p.lq + kTileQ - 1) / kTileQ, p.heads * p.v_slices, p.batch);
+  CA_KERNEL_LAUNCH(kern, grid, kAttnThreads, Cfg::kSmemBytes, stream, q, k, v, p);
   return cudaGetLastError();
 }
 
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p,
                              cudaStream_t stream) {
-  // developer knobs: CA_ATTN_SPLIT = softmax warpgroups per CTA (1 = one thread per row as in round 1, 2 = two);
-  // CA_ATTN_POLY = share of exponentials moved off the MUFU pipe (eighths)
-  static const int split = getenv("CA_ATTN_SPLIT") ? atoi(getenv("CA_ATTN_SPLIT")) : kSplitDefault;
-  static const int poly = getenv("CA_ATTN_POLY") ? atoi(getenv("CA_ATTN_POLY")) : kPolyDefault;
-  // CA_ATTN_THROTTLE = column pairs per dependency group of the exp schedule throttle (0 = off; 4 or 8)
-  static const int th = getenv("CA_ATTN_THROTTLE") ? atoi(getenv("CA_ATTN_THROTTLE")) : kThrottleDefault;
-  // CA_ATTN_SHORT=0: developer A/B switch, sends Lk <= 80 through the general kernel as before
-  static const bool short_kv = !(getenv("CA_ATTN_SHORT") && getenv("CA_ATTN_SHORT")[0] == '0');
-  if (short_kv && p.dqk_chunks == 1 && p.lk >= 1 && p.lk <= kShortKV) return launch_short<kPolyDefault>(q, k, v, p, stream);
   switch (p.dqk_chunks) {
-    case 1:
-      if (split == 1) {
-        if (th == 2) return poly == 3 ? launch_dq<1, 3, 1, 2>(q, k, v, p, stream) : launch_dq<1, kPolyDefault, 1, 2>(q, k, v, p, stream);
-        if (th == 4) return poly == 3 ? launch_dq<1, 3, 1, 4>(q, k, v, p, stream) : launch_dq<1, kPolyDefault, 1, 4>(q, k, v, p, stream);
-        if (th == 8) return poly == 3 ? launch_dq<1, 3, 1, 8>(q, k, v, p, stream) : launch_dq<1, kPolyDefault, 1, 8>(q, k, v, p, stream);
-        return launch_dq<1, kPolyDefault, 1>(q, k, v, p, stream);
-      }
-      switch (poly) {
-        case 0: return launch_dq<1, 0, 2>(q, k, v, p, stream);
-        case 3: return launch_dq<1, 3, 2>(q, k, v, p, stream);
-        case 4: return launch_dq<1, 4, 2>(q, k, v, p, stream);
-        default: return launch_dq<1, kPolyDefault, 2>(q, k, v, p, stream);
-      }
-    case 2: return split == 1 ? launch_dq<2, kPolyDefault, 1>(q, k, v, p, stream) : launch_dq<2, kPolyDefault, 2>(q, k, v, p, stream);
-    case 3: return split == 1 ? launch_dq<3, kPolyDefault, 1>(q, k, v, p, stream) : launch_dq<3, kPolyDefault, 2>(q, k, v, p, stream);
+    case 1: return launch_dq<1>(q, k, v, p, stream);
+    case 2: return launch_dq<2>(q, k, v, p, stream);
+    case 3: return launch_dq<3>(q, k, v, p, stream);
     default: return cudaErrorInvalidValue;
   }
 }

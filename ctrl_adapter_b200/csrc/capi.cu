@@ -70,8 +70,8 @@ int num_sms() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -103,7 +103,7 @@ int ca_device_ok(void) {
   int dev = 0, major = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return fail(CA_ERR_UNSUPPORTED, "device compute capability %d.x, need 10.x (sm_100a)", major);
+  if (major != 9) return fail(CA_ERR_UNSUPPORTED, "device compute capability %d.x, need 9.x (sm_90a)", major);
   return CA_OK;
 }
 
@@ -131,23 +131,8 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
     else if (d->w_rows <= 128) bn = 128;
     else bn = 256;
   }
-  // 256 x 320 pair tiles (csrc/gemm_conv_wide.cu) where the N = 320 / 640 / 960 / 1920 GEMMs would otherwise use 160-wide
-  // ones (L2-feed bound); only for the bias / bias+residual epilogues, CTA pairs, bf16 output.  Default since round 2
-  // (kernel checks green on hardware, 181.8 -> 179.7 ms / SDXL step); CA_GEMM_BN320=0 restores the 160-wide tiles.
-  static const bool wide_ok = !(getenv("CA_GEMM_BN320") && getenv("CA_GEMM_BN320")[0] == '0') &&
-                              getenv("CA_GEMM_1CTA") == nullptr;
-  // ... and only for long contractions: its two-half tiles pay off from ~24 k-blocks on (3x3 convolutions, K >= 1920
-  // linears: +5..9 %); for the thin GEMMs of the video backbones (K = 320 .. 1280) the 160-wide kernel is 4..60 % faster
-  // (profiles/r2_experiments.md, "BN = 320 dispatch threshold")
-  const long long k_total = static_cast<long long>(d->ntaps) * d->w_k_per_tap;
-  static const long long wide_min_k = getenv("CA_GEMM_BN320_MINK") ? atoll(getenv("CA_GEMM_BN320_MINK")) : 1536;  // A/B knob
-  if (wide_ok && k_total >= wide_min_k && d->bn == 0 && bn == 160 && d->w_rows % 320 == 0 && d->act == CA_ACT_NONE && !d->out_fp32 &&
-      d->out_scale == 1.0f && d->blend_src == nullptr && (d->rowvec == nullptr || d->residual == nullptr) &&
-      reinterpret_cast<uintptr_t>(d->bias) % 16 == 0)
-    bn = 320;
+  if (bn != 64 && bn != 128 && bn != 160 && bn != 256) return fail(CA_ERR_INVALID, "bn must be 0, 64, 128, 160 or 256");
   if (geglu && (d->w_rows % bn) != 0) return fail(CA_ERR_INVALID, "GEGLU needs w_rows %% bn == 0");
-  // CTA pairs (tcgen05 cta_group::2, M = 256 per pair) unless CA_GEMM_1CTA is set (A/B comparison / debugging)
-  static const int ncta = getenv("CA_GEMM_1CTA") ? 1 : 2;
 
   int k_per_tap = 0;
   for (int s = 0; s < d->nsrc; ++s) {
@@ -212,17 +197,16 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
     if (ktot % 8 != 0) return fail(CA_ERR_INVALID, "weight row length must be a multiple of 8");
     cuuint64_t dims[2] = {ktot, static_cast<cuuint64_t>(d->w_rows)};
     cuuint64_t strides[1] = {ktot * 2};
-    // each CTA of a pair stages half of the N tile (as two 80-row chunks for the 320-wide experiment)
-    cuuint32_t box[2] = {64, static_cast<cuuint32_t>(bn == 320 ? 80 : bn / ncta)};
+    cuuint32_t box[2] = {64, static_cast<cuuint32_t>(bn)};
     int rc = make_tmap(&tw, d->w, 2, dims, strides, box);
     if (rc) return rc;
   }
   const long long tiles_m = static_cast<long long>(p.ntile[0]) * p.ntile[1] * p.ntile[2] * p.ntile[3];
-  const long long tiles = ((tiles_m + ncta - 1) / ncta) * p.n_tiles_n;  // tiles per CTA group
+  const long long tiles = tiles_m * p.n_tiles_n;
   if (tiles <= 0) return fail(CA_ERR_INVALID, "empty problem");
-  const long long max_groups = num_sms() / ncta;
-  const int grid = static_cast<int>((tiles < max_groups ? tiles : max_groups) * ncta);
-  CA_LAUNCH(ca::launch_gemm_conv(bn, ncta, ta[0], ta[1], tw, p, grid, stream), "gemm_conv launch");
+  const long long sms = num_sms();
+  const int grid = static_cast<int>(tiles < sms ? tiles : sms);
+  CA_LAUNCH(ca::launch_gemm_conv(bn, ta[0], ta[1], tw, p, grid, stream), "gemm_conv launch");
 }
 
 int ca_attention(const ca_attention_desc* d, void* cuda_stream) {
@@ -254,11 +238,6 @@ int ca_attention(const ca_attention_desc* d, void* cuda_stream) {
   ca::AttnParams p;
   p.batch = d->batch; p.heads = d->heads; p.lq = d->lq; p.lk = d->lk;
   p.kv_batch_div = kv_div;
-  p.trace = trace_ptr();
-  static const unsigned stagger = getenv("CA_ATTN_STAGGER") ? static_cast<unsigned>(atoi(getenv("CA_ATTN_STAGGER"))) : 0u;
-  p.stagger_ns = stagger;
-  static const unsigned backoff = getenv("CA_ATTN_BACKOFF") ? static_cast<unsigned>(atoi(getenv("CA_ATTN_BACKOFF"))) : 64u;
-  p.backoff_ns = backoff;
   p.dqk_chunks = d->head_dim_pad / 64;
   p.v_slices = d->head_dim_pad / 64;
   p.scale_log2 = d->scale * 1.4426950408889634f;

@@ -1,7 +1,6 @@
-// Blackwell (sm_100a) primitives shared by the hot-path kernels: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) wrappers and the
-// UMMA shared-memory / instruction descriptors.  Hand-written inline PTX; no
-// CUTLASS / CuTe dependency.
+// Hopper (sm_90a) primitives shared by the hot-path kernels: mbarrier, TMA
+// (cp.async.bulk.tensor), wgmma fences / commits and the wgmma shared-memory
+// matrix descriptor.  Hand-written inline PTX; no CUTLASS / CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -49,7 +48,7 @@ __device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
 __device__ __forceinline__ float bf16lo_to_float(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi_to_float(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
 
-// ---- packed fp32x2 arithmetic (FFMA2 / FADD2: two lanes per issued instruction) ----
+// ---- fp32 pairs kept in one 64-bit value (per-lane IEEE fma / add / mul, round to nearest) ----
 __device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -59,19 +58,23 @@ __device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack_f32x2(a, a0, a1);
+  unpack_f32x2(b, b0, b1);
+  unpack_f32x2(c, c0, c1);
+  return pack_f32x2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack_f32x2(a, a0, a1);
+  unpack_f32x2(b, b0, b1);
+  return pack_f32x2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack_f32x2(a, a0, a1);
+  unpack_f32x2(b, b0, b1);
+  return pack_f32x2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 
 __device__ __forceinline__ bool elect_one() {
@@ -166,216 +169,51 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
-// ----------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (K-major, 16-bit elements packed two per 32-bit TMEM cell, one row per
-// lane) is read straight from tensor memory -- used for P in softmax(QK^T) V so P never touches shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// registers -> TMEM (32 lanes x 32 columns); used to rescale the attention output accumulator in place
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-// registers -> TMEM, 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-// registers -> TMEM, 32 lanes x 8 columns
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants.  Inside a 2-CTA cluster the shared::cluster address of a CTA's own shared
-// memory carries the CTA's rank in bit 24; clearing it addresses the same offset in the leader (rank 0) CTA.
-// ----------------------------------------------------------------------------
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same offset in the leader CTA of the pair (works from either CTA)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  // .relaxed: a .release at cluster scope is compiled to MEMBAR.ALL.GPU, which stalls the arriving warp until all of
-  // its global stores have been acknowledged (2-3k cycles per tile in the GEMM epilogue).  The only thing ordered
-  // through these barriers is TMEM traffic, which tcgen05.wait + tcgen05.fence::before_thread_sync already order.
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-// TMA loads issued by either CTA of a pair; completion bytes are credited to the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                 int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-      "r"(c4)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// commit of the leader's MMAs: arrives on the mbarrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// D[tmem, 256 rows over the CTA pair] (+)= A * B, issued by ONE thread of the leader CTA
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 16-byte asynchronous global -> shared copy (LDGSTS), used to prefetch residual tiles for the epilogue
+// 16-byte asynchronous global -> shared copy (LDGSTS)
 __device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: PTX ISA "tcgen05 matrix / instruction descriptor")
+// wgmma (Hopper warpgroup MMA): fences, commit / wait, shared-memory matrix descriptor
 // ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128B swizzle. `saddr` = byte address in the
-// shared window (tile base must be 1024B aligned; K-advance inside the swizzle
-// atom is done by adding bytes to the start address).
+// orders register / shared-memory writes of the warpgroup before the wgmma.mma_async that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Shared-memory matrix descriptor, 128B swizzle (the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B).  `saddr` =
+// byte address in the shared window (tile base 1024B aligned; a K-advance inside the 128-byte swizzle row is done by
+// adding bytes to the start address).
 //   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+//   bits [32,46) stride byte offset >> 4 bits [62,64) layout type: 1 = SWIZZLE_128B
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= 1ull << 62;
   return d;
 }
-// Instruction descriptor for kind::f16, A/B = bf16, D = fp32.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt (1=bf16)
-//   [15] A major (0=K)   [16] B major (0=K, 1=MN)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
-}
+
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 }  // namespace ca
 
 // ---------------------------------------------------------------------------------------------------------------
-// Programmatic dependent launch (default since round 2: 181.8 -> 175.8 ms / SDXL step, profiles/r2_experiments.md;
-// -DCA_NO_PDL builds without it, see scripts/build_variants.py).
-// With ~1500 launches per step, every kernel's prologue (barrier init, TMEM allocation, descriptor prefetch) and the
+// Programmatic dependent launch (-DCA_NO_PDL builds without it).
+// With ~1500 launches per step, every kernel's prologue (barrier init, descriptor prefetch) and the
 // launch latency itself sit between the tail of one kernel and the first useful cycle of the next.  With PDL each
 // kernel (a) tells the scheduler right away that its dependents may be launched as SMs free up and (b) waits for the
 // previous grid's completion only after its own prologue, before the first global-memory access.  Without the launch
@@ -409,7 +247,7 @@ inline cudaError_t launch_pdl(K kernel, dim3 grid, dim3 block, size_t smem, cuda
 #define CA_KERNEL_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #endif
 
-// Developer instrumentation (scripts/gemm_trace.py): cycles each role of a kernel spends blocked, 16 counters per CTA
+// Developer instrumentation: cycles each role of a kernel spends blocked, 16 counters per CTA
 // written through the `trace` pointer of the kernel's Params struct.  Compiled out unless -DCA_TRACE.
 #ifdef CA_TRACE
 #define TR_CTA() (blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z))

@@ -1,15 +1,11 @@
-// Host-side dispatch of gemm_conv_kernel: picks the epilogue specialisation from the runtime parameters and forwards to
-// the per-BN translation units (gemm_conv_bn*.cu; split so the ~20 kernel instantiations compile in parallel).
-#include <cstdint>
-
+// Host-side dispatch of gemm_conv_kernel to the per-BN translation units (gemm_conv_bn*.cu; split so the kernel
+// instantiations compile in parallel).
 #include "kernels.h"
 
 namespace ca {
 
-enum { EPI_GENERIC = 0, EPI_PLAIN = 1, EPI_RES = 2, EPI_GEGLU = 3 };  // mirrors gemm_conv_kernel.cuh
-
-#define CA_DECL_BN(bn)                                                                                             \
-  cudaError_t launch_gemm_bn##bn(int ncta, int epi, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, \
+#define CA_DECL_BN(bn)                                                                                         \
+  cudaError_t launch_gemm_bn##bn(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,           \
                                  const GemmParams& p, int grid, cudaStream_t stream);
 CA_DECL_BN(64)
 CA_DECL_BN(128)
@@ -17,39 +13,13 @@ CA_DECL_BN(160)
 CA_DECL_BN(256)
 #undef CA_DECL_BN
 
-cudaError_t launch_gemm_conv(int bn, int ncta, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
-                             const GemmParams& p_in, int grid, cudaStream_t stream) {
-  GemmParams p = p_in;
-  int epi = EPI_GENERIC;
-  // the lean epilogues read the fp32 bias with 16-byte loads and move 8-column groups
-  const bool vec_ok = (reinterpret_cast<uintptr_t>(p.bias) % 16 == 0) && (p.n_out % 8 == 0);
-  if (ncta == 2 && vec_ok && !p.out_fp32 && p.out_scale == 1.0f && p.blend_src == nullptr) {
-    if (p.act == CA_ACT_GEGLU) {
-      if (p.rowvec == nullptr && p.residual == nullptr && bn == 256) epi = EPI_GEGLU;
-    } else if (p.act == CA_ACT_NONE) {
-      if (p.rowvec == nullptr && p.residual == nullptr) {
-        epi = EPI_PLAIN;
-      } else if (p.rowvec == nullptr) {
-        epi = EPI_RES;
-      } else if (p.residual == nullptr) {
-        // a broadcast row vector (the resnet's time-embedding add) is a residual whose spatial strides are zero
-        bool aligned = reinterpret_cast<uintptr_t>(p.rowvec) % 16 == 0;  // rows are fetched with 16-byte cp.async
-        for (int i = 0; i < 4; ++i) aligned = aligned && (p.vstride[i] % 8 == 0);
-        if (aligned) {
-          epi = EPI_RES;
-          p.residual = p.rowvec;
-          for (int i = 0; i < 4; ++i) p.rstride[i] = p.vstride[i];
-          p.rowvec = nullptr;
-        }
-      }
-    }
-  }
+cudaError_t launch_gemm_conv(int bn, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
+                             const GemmParams& p, int grid, cudaStream_t stream) {
   switch (bn) {
-    case 64: return launch_gemm_bn64(ncta, epi, a0, a1, w, p, grid, stream);
-    case 128: return launch_gemm_bn128(ncta, epi, a0, a1, w, p, grid, stream);
-    case 160: return launch_gemm_bn160(ncta, epi, a0, a1, w, p, grid, stream);
-    case 256: return launch_gemm_bn256(ncta, epi, a0, a1, w, p, grid, stream);
-    case 320: return ncta == 2 ? launch_gemm_wide(epi, a0, a1, w, p, grid, stream) : cudaErrorInvalidValue;
+    case 64: return launch_gemm_bn64(a0, a1, w, p, grid, stream);
+    case 128: return launch_gemm_bn128(a0, a1, w, p, grid, stream);
+    case 160: return launch_gemm_bn160(a0, a1, w, p, grid, stream);
+    case 256: return launch_gemm_bn256(a0, a1, w, p, grid, stream);
     default: return cudaErrorInvalidValue;
   }
 }

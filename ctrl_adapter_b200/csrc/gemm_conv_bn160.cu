@@ -1,9 +1,9 @@
-// gemm_conv_kernel instantiations for BN = 160 (see gemm_conv.cu for the dispatch).
+// gemm_conv_kernel instantiation for BN = 160 (see gemm_conv.cu for the dispatch).
 #include "gemm_conv_kernel.cuh"
 
 namespace ca {
-cudaError_t launch_gemm_bn160(int ncta, int epi, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
-                              const GemmParams& p, int grid, cudaStream_t stream) {
-  return launch_bn<160>(ncta, epi, a0, a1, w, p, grid, stream);
+cudaError_t launch_gemm_bn160(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
+                              int grid, cudaStream_t stream) {
+  return launch_bn<160>(a0, a1, w, p, grid, stream);
 }
 }  // namespace ca

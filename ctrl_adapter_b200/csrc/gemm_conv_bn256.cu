@@ -1,9 +1,9 @@
-// gemm_conv_kernel instantiations for BN = 256 (see gemm_conv.cu for the dispatch).
+// gemm_conv_kernel instantiation for BN = 256 (see gemm_conv.cu for the dispatch).
 #include "gemm_conv_kernel.cuh"
 
 namespace ca {
-cudaError_t launch_gemm_bn256(int ncta, int epi, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
-                              const GemmParams& p, int grid, cudaStream_t stream) {
-  return launch_bn<256>(ncta, epi, a0, a1, w, p, grid, stream);
+cudaError_t launch_gemm_bn256(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
+                              int grid, cudaStream_t stream) {
+  return launch_bn<256>(a0, a1, w, p, grid, stream);
 }
 }  // namespace ca

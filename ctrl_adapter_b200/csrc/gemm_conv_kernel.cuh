@@ -1,4 +1,4 @@
-// Multi-tap tcgen05 GEMM: the one contraction kernel behind every Linear, 1x1 / 3x3
+// Multi-tap wgmma GEMM: the one contraction kernel behind every Linear, 1x1 / 3x3
 // (stride 1 or 2) Conv2d and (3,1,1) temporal Conv3d on the denoising hot path.
 //
 //   out[row, n] = epilogue( sum_{tap} sum_{src} sum_{c} A_src[row + off(tap), c] * W[n, tap, src, c] )
@@ -8,77 +8,42 @@
 // hardware zero fill outside the tensor -- implicit-GEMM convolution with no im2col buffer.  Weights are
 // [N][taps*K] bf16 (K contiguous).
 //
-// NCTA == 2 (default): CTA pairs (cluster 2x1x1) issue tcgen05.mma.cta_group::2 with M = 256: each CTA stages its
-// own 128 A rows and HALF of the BN weight rows, which cuts the L2 -> shared-memory traffic per MMA by a third
-// (the kernel is L2-bandwidth bound with 1-CTA tiles); accumulators live in both CTAs' TMEM (128 lanes each).
-// NCTA == 1: single-CTA 128 x BN tiles (kept for A/B comparison: CA_GEMM_1CTA=1).
-//
-// Per CTA (persistent, warp specialised, 384 threads):
-//   warp 0    : TMA producer  (A box + its share of the W tile per k-iteration into a multi-stage smem ring;
-//               completion bytes of both CTAs are credited to the leader's "full" mbarrier)
-//   warp 1    : MMA issuer    (leader CTA only; one thread; commits are multicast to both CTAs' barriers)
-//   warp 2    : TMEM allocator
-//   warps 4-11: epilogue.  Warp e owns TMEM lane quarter (e & 3) and every second 64-column unit (e >> 2):
-//               residual tile prefetched with cp.async -> tcgen05.ld -> bias / SiLU / GEGLU / scale / temb / residual /
-//               blend (bf16 rounding after each step = the autocast rounding points) -> warp-private swizzled smem
-//               staging -> 128-byte coalesced global stores.
-// Accumulators are double buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
-//
-// The epilogue is specialised at compile time (EPI): with 4-5 tiles per CTA and K as small as 320 the epilogue's
-// instruction count, not the tensor pipe, bounds many of the UNet's GEMMs, so the three shapes that carry ~all of the
-// time get lean code paths and everything else goes through the generic one:
-//   EPI_PLAIN  : bias                                   (attention projections, conv_in/out, ControlNet convs)
-//   EPI_RES    : bias -> round -> + residual-like tile  (attn/ff out-proj + skip, resnet conv2 + skip, conv1 + temb)
-//   EPI_GEGLU  : value/gate bias -> erf-GELU -> product (FeedForward proj_in)
-//   EPI_GENERIC: any combination of SiLU / scale / row vector / residual / AlphaBlender / fp32 output
+// Per CTA (persistent over 128 x BN tiles, warp specialised, 384 threads = 3 warpgroups):
+//   warpgroup 0, one thread : TMA producer (A box + W tile per k-iteration into a multi-stage shared-memory ring)
+//   warpgroups 1, 2         : consumers.  Warpgroup g issues m64nBNk16 wgmma for rows [64g, 64g + 64) of the tile with
+//                             both operands read from the 128B-swizzled ring, accumulates in registers, and releases
+//                             a ring slot as soon as the wgmma that read it have retired.  Then the epilogue straight
+//                             from the accumulator registers: bias / SiLU / GEGLU / scale / row vector / residual /
+//                             AlphaBlender / fp32 output, with a bf16 rounding after each step (the autocast rounding
+//                             points of the reference).
+// setmaxnreg moves registers from the producer warpgroup to the consumers (BN = 256: 128 accumulators per thread).
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace ca {
 
-enum { EPI_GENERIC = 0, EPI_PLAIN = 1, EPI_RES = 2, EPI_GEGLU = 3 };
-
 static constexpr int kBM = 128;
 static constexpr int kBK = 64;
-static constexpr int kEpiWarps = 8;
-static constexpr int kGemmThreads = 128 + kEpiWarps * 32;  // 384
-static constexpr uint32_t kStageRowBytes = 128;            // 64 bf16 columns per staged row
-static constexpr uint32_t kWarpStageBytes = 32 * kStageRowBytes;           // 4 KB
-static constexpr uint32_t kStagingBytes = 2 * kEpiWarps * kWarpStageBytes;  // out + residual-in: 64 KB
+static constexpr int kGemmThreads = 384;
 
-template <int BN, int NCTA>
+template <int BN>
 struct GemmCfg {
-  static constexpr uint32_t kABytes = kBM * kBK * 2;       // 16 KB
-  static constexpr uint32_t kBRows = BN / NCTA;             // weight rows staged by this CTA
-  static constexpr uint32_t kBBytes = kBRows * kBK * 2;
+  static constexpr uint32_t kABytes = kBM * kBK * 2;  // 16 KB
+  static constexpr uint32_t kBBytes = BN * kBK * 2;   // a multiple of the 1 KB swizzle atom for every BN used
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  static constexpr uint32_t kBudget = 232448 - 1024 - 256 - kStagingBytes;
+  static constexpr uint32_t kBudget = 232448 - 1024 - 256;  // 227 KB per block on H100, minus alignment and barriers
   static constexpr int kStagesRaw = kBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr uint32_t kTmemCols = (BN <= 64) ? 128 : (BN <= 128 ? 256 : 512);  // 2 accumulator stages
-  static constexpr uint32_t kAccStride = kTmemCols / 2;
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// erf with |error| <= 1.5e-7 (Abramowitz & Stegun 7.1.26) -- far below the bf16 rounding applied to GELU's output
-__device__ __forceinline__ float fast_erf(float x) {
-  const float ax = fabsf(x);
-  float t;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f, ax, 1.0f)));
-  float p = fmaf(1.061405429f, t, -1.453152027f);
-  p = fmaf(p, t, 1.421413741f);
-  p = fmaf(p, t, -0.284496736f);
-  p = fmaf(p, t, 0.254829592f);
-  const float e = 1.0f - p * t * __expf(-ax * ax);
-  return copysignf(e, x);
-}
-
-// exact-erf GELU of a bf16-valued x, same erf approximation, arranged as relu(x) - |x| * q(|x|) with
-// q = 0.5 * erfc(|x| / sqrt 2): 11 FMA/ALU + 2 MUFU instructions, no branches
+// exact-erf GELU of a bf16-valued x (erf of Abramowitz & Stegun 7.1.26, |error| <= 1.5e-7), arranged as
+// relu(x) - |x| * q(|x|) with q = 0.5 * erfc(|x| / sqrt 2): no cancellation for negative x, no branches
 __device__ __forceinline__ float gelu_erf(float x) {
   const float a = fabsf(x);
-  float t;  // MUFU.RCP (1 ulp): __frcp_rn costs a Newton step, a range check and a slow-path call per element
+  float t;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f * 0.70710678118654752440f, a, 1.0f)));
   float p = fmaf(0.5f * 1.061405429f, t, 0.5f * -1.453152027f);
   p = fmaf(p, t, 0.5f * 1.421413741f);
@@ -91,598 +56,248 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(-a, q, fmaxf(x, 0.0f));
 }
 
-template <int BN, int NCTA, int EPI>
+// the epilogue after bias / activation of two adjacent columns (col, col + 1) of one row; `nv` of them exist
+__device__ __forceinline__ void gemm_finish_pair(const GemmParams& p, float v0, float v1, int col, int nv,
+                                                 long long out_off, long long res_off, long long rv_off,
+                                                 float alpha_s, float alpha_t) {
+  if (p.out_scale != 1.0f) {
+    v0 *= p.out_scale;
+    v1 *= p.out_scale;
+    if (!p.out_fp32) round2_bf16(v0, v1);  // fp32 output (attention scores of the VAE): unrounded
+  }
+  if (p.rowvec != nullptr) {
+    const __nv_bfloat16* rv = p.rowvec + rv_off + col;
+    v0 = round_bf16(v0 + __bfloat162float(rv[0]));
+    if (nv > 1) v1 = round_bf16(v1 + __bfloat162float(rv[1]));
+  }
+  if (p.out_fp32) {
+    float* op = reinterpret_cast<float*>(p.out) + out_off + col;
+    if (p.residual != nullptr) {
+      v0 += __bfloat162float(p.residual[res_off + col]);
+      if (nv > 1) v1 += __bfloat162float(p.residual[res_off + col + 1]);
+    }
+    op[0] = v0;
+    if (nv > 1) op[1] = v1;
+    return;
+  }
+  if (p.residual != nullptr) {
+    const __nv_bfloat16* rs = p.residual + res_off + col;
+    v0 += __bfloat162float(rs[0]);
+    v1 += __bfloat162float(rs[1]);
+    round2_bf16(v0, v1);
+  }
+  if (p.blend_src != nullptr) {
+    const __nv_bfloat16* bs = p.blend_src + res_off + col;
+    v0 = round_bf16(round_bf16(alpha_s * __bfloat162float(bs[0])) + round_bf16(alpha_t * v0));
+    v1 = round_bf16(round_bf16(alpha_s * __bfloat162float(bs[1])) + round_bf16(alpha_t * v1));
+  }
+  __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + out_off + col;
+  if ((reinterpret_cast<uintptr_t>(op) & 3) == 0) {
+    *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
+  } else {
+    op[0] = __float2bfloat16_rn(v0);
+    op[1] = __float2bfloat16_rn(v1);
+  }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1,
                  const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
-  using Cfg = GemmCfg<BN, NCTA>;
+  using Cfg = GemmCfg<BN>;
   CA_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
 
-  uint8_t* smem_a = smem;                                         // kStages x 16 KB
-  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;           // kStages x kBRows*128 B
-  uint8_t* smem_stage = smem + Cfg::kStages * Cfg::kStageBytes;   // epilogue staging (out, residual-in)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stage + kStagingBytes);
-  uint64_t* full_bar = bars;                     // [kStages]   (the leader's instance is the live one)
-  uint64_t* empty_bar = bars + Cfg::kStages;     // [kStages]
-  uint64_t* acc_full = bars + 2 * Cfg::kStages;  // [2]
-  uint64_t* acc_empty = acc_full + 2;            // [2]         (leader's instance)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint8_t* smem_a = smem;                                // kStages x 16 KB
+  uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;  // kStages x BN*128 B
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* full_bar = bars;                  // [kStages]
+  uint64_t* empty_bar = bars + Cfg::kStages;  // [kStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int rank = (NCTA == 2) ? static_cast<int>(cluster_ctarank()) : 0;
-  const bool leader = rank == 0;
-  const int group = blockIdx.x / NCTA;          // CTA (pair) index
-  const int ngroups = gridDim.x / NCTA;
 
   const int tiles_m = p.ntile[0] * p.ntile[1] * p.ntile[2] * p.ntile[3];
-  const int tiles_mg = (tiles_m + NCTA - 1) / NCTA;  // M tiles per CTA group
-  const int total_tiles = tiles_mg * p.n_tiles_n;
+  const int total_tiles = tiles_m * p.n_tiles_n;
   const int chunks0 = (p.src_c[0] + kBK - 1) / kBK;
   const int chunks1 = (p.nsrc > 1) ? (p.src_c[1] + kBK - 1) / kBK : 0;
   const int kiters = p.ntaps * (chunks0 + chunks1);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a0);
     if (p.nsrc > 1) tma_prefetch_desc(&tmap_a1);
     tma_prefetch_desc(&tmap_w);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1);
-      mbar_init(&acc_empty[a], NCTA * kEpiWarps);  // one arrive per epilogue warp of every CTA of the group
+      mbar_init(&empty_bar[s], 8);  // one arrive per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (NCTA == 2) tmem_alloc_pair<Cfg::kTmemCols>(tmem_slot);
-    else tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (NCTA == 2) cluster_sync_all();  // peer barriers initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   CA_PDL_WAIT();  // prologue done: the previous kernel's output (A, residual, bias ...) may be read from here on
 
-  // decode tile -> (n tile, this CTA's 4-D M tile origin)
+  // decode tile -> (n tile, 4-D M tile origin)
   auto tile_coords = [&](int tile, int& tn, int (&org)[4]) {
     tn = tile % p.n_tiles_n;
-    int tm = (tile / p.n_tiles_n) * NCTA + rank;  // may be == tiles_m for the last odd tile: fully out of range
+    int tm = tile / p.n_tiles_n;
     org[0] = (tm % p.ntile[0]) * p.box[0]; tm /= p.ntile[0];
     org[1] = (tm % p.ntile[1]) * p.box[1]; tm /= p.ntile[1];
     org[2] = (tm % p.ntile[2]) * p.box[2]; tm /= p.ntile[2];
     org[3] = tm * p.box[3];
   };
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      TR_DECL(tr_wait_empty);
-      [[maybe_unused]] const long long tr_start = TR_NOW();
-      for (int tile = group; tile < total_tiles; tile += ngroups) {
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int tn, org[4];
         tile_coords(tile, tn, org);
-        const int n0 = tn * BN + rank * static_cast<int>(Cfg::kBRows);
+        const int n0 = tn * BN;
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const int c1 = org[0] + p.tap_off[tap][0], c2 = org[1] + p.tap_off[tap][1];
           const int c3 = org[2] + p.tap_off[tap][2], c4 = org[3] + p.tap_off[tap][3];
           const int kbase = tap * p.k_per_tap;
           for (int ch = 0; ch < chunks0 + chunks1; ++ch) {
-            TR_WAIT(tr_wait_empty, mbar_wait(&empty_bar[stage], phase ^ 1));
+            mbar_wait(&empty_bar[stage], phase ^ 1);
             const bool second = ch >= chunks0;
             const int cc = (second ? (ch - chunks0) : ch) * kBK;
             const int ca = cc + (second ? p.src_c0_off[1] : p.src_c0_off[0]) + p.tap_c_off[tap];
             const int kw = kbase + (second ? p.src_c[0] : 0) + cc;
             const CUtensorMap* ta = second ? &tmap_a1 : &tmap_a0;
-            if (NCTA == 2) {
-              if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-              tma_load_5d_pair(smem_a + stage * Cfg::kABytes, ta, &full_bar[stage], ca, c1, c2, c3, c4);
-              tma_load_2d_pair(smem_b + stage * Cfg::kBBytes, &tmap_w, &full_bar[stage], kw, n0);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-              tma_load_5d(smem_a + stage * Cfg::kABytes, ta, &full_bar[stage], ca, c1, c2, c3, c4);
-              tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_w, &full_bar[stage], kw, n0);
-            }
+            mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+            tma_load_5d(smem_a + stage * Cfg::kABytes, ta, &full_bar[stage], ca, c1, c2, c3, c4);
+            tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_w, &full_bar[stage], kw, n0);
             if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
           }
         }
       }
-      TR_PUT(0, TR_NOW() - tr_start);
-      TR_PUT(1, tr_wait_empty);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kBM * NCTA, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      TR_DECL(tr_wait_full);
-      TR_DECL(tr_wait_acc);
-      [[maybe_unused]] const long long tr_start = TR_NOW();
-      for (int tile = group; tile < total_tiles; tile += ngroups) {
-        TR_WAIT(tr_wait_acc, mbar_wait(&acc_empty[acc], acc_phase ^ 1));
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccStride;
-        for (int it = 0; it < kiters; ++it) {
-          TR_WAIT(tr_wait_full, mbar_wait(&full_bar[stage], phase));
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * Cfg::kABytes);
-          const uint32_t b_addr = smem_u32(smem_b + stage * Cfg::kBBytes);
+    return;
+  }
+
+  // ===================== consumers: wgmma main loop + register epilogue =====================
+  setmaxnreg_inc<232>();
+  const int cw = (warp >> 2) - 1;   // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+  const int wq = warp & 3;          // warp inside the warpgroup: rows [16 wq, 16 wq + 16) of those
+  const bool geglu = (p.act == CA_ACT_GEGLU);
+  float alpha_s = 0.f, alpha_t = 0.f;
+  if (p.blend_src != nullptr) {
+    const float a = *p.blend_alpha;  // bf16-valued
+    alpha_s = a;
+    alpha_t = round_bf16(1.0f - a);
+  }
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int tn, org[4];
+    tile_coords(tile, tn, org);
+    int prev = -1;
+    for (int it = 0; it < kiters; ++it) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(smem_a + stage * Cfg::kABytes) + cw * 64 * 128;
+      const uint32_t b_addr = smem_u32(smem_b + stage * Cfg::kBBytes);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            const uint64_t da = umma_smem_desc_sw128(a_addr + k * 32, 16, 1024);
-            const uint64_t db = umma_smem_desc_sw128(b_addr + k * 32, 16, 1024);
-            if (NCTA == 2) umma_bf16_ss_pair(d_tmem, da, db, idesc, (it | k) != 0 ? 1u : 0u);
-            else umma_bf16_ss(d_tmem, da, db, idesc, (it | k) != 0 ? 1u : 0u);
-          }
-          // frees the smem slot (in both CTAs) when the MMAs above retire
-          if (NCTA == 2) umma_commit_pair(&empty_bar[stage]); else umma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        if (NCTA == 2) umma_commit_pair(&acc_full[acc]); else umma_commit(&acc_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      for (int k = 0; k < kBK / 16; ++k) {
+        Wgmma<BN>::ss(acc, gmma_desc_sw128(a_addr + k * 32, 16, 1024), gmma_desc_sw128(b_addr + k * 32, 16, 1024),
+                      (it | k) != 0 ? 1 : 0);
       }
-      TR_PUT(2, tr_wait_full);
-      TR_PUT(3, tr_wait_acc);
-      TR_PUT(8, TR_NOW() - tr_start);
+      wgmma_commit();
+      if (prev >= 0) {
+        wgmma_wait<1>();  // the wgmma of the previous k-iteration retired: its ring slot may be refilled
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int ew = warp - 4;           // 0..7
-    const int q = warp & 3;            // TMEM lane quarter this warp may access (== warp id % 4)
-    const int half_sel = ew >> 2;      // which of every two 64-column units this warp processes
-    const int r = q * 32 + lane;       // tile row owned by this thread
-    const bool geglu = (p.act == CA_ACT_GEGLU);
-    const int ncols_out = geglu ? BN / 2 : BN;  // output columns produced per tile
-    // warp-private [32 rows][128 B] buffers, 16-byte units XOR-swizzled with (row & 7)
-    uint8_t* stg_out = smem_stage + ew * kWarpStageBytes;
-    uint8_t* stg_res = smem_stage + (kEpiWarps + ew) * kWarpStageBytes;
-    const bool use_res = p.residual != nullptr && !p.out_fp32;
-    const bool plain = !geglu && p.act == CA_ACT_NONE && p.out_scale == 1.0f && p.rowvec == nullptr &&
-                       p.residual == nullptr && p.blend_src == nullptr && !p.out_fp32;
-    float alpha_s = 0.f, alpha_t = 0.f;
-    if (p.blend_src != nullptr) {
-      const float a = *p.blend_alpha;  // bf16-valued
-      alpha_s = a;
-      alpha_t = round_bf16(1.0f - a);
-    }
-    // copy-in / copy-out role of this lane: row (it*4 + lane/8) of the warp's 32 rows, 16-byte segment lane%8
-    const int seg = lane & 7;
-    const int rsub = lane >> 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    TR_DECL(tr_wait_accfull);
-    TR_DECL(tr_wait_cp);
-    TR_DECL(tr_arrive);
-    TR_DECL(tr_tmem);
-    TR_DECL(tr_tiles);
-    [[maybe_unused]] const long long tr_start = TR_NOW();
-    for (int tile = group; tile < total_tiles; tile += ngroups) {
-      int tn, org[4];
-      tile_coords(tile, tn, org);
-      int rr = r;
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    // ---- epilogue: thread holds rows (r0, r0 + 8) x columns 8 j + 2 (lane & 3) + {0, 1} ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      int rr = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;
       const int i1 = rr % p.box[0]; rr /= p.box[0];
       const int i2 = rr % p.box[1]; rr /= p.box[1];
       const int i3 = rr % p.box[2]; rr /= p.box[2];
       const int i4 = rr;
       const int o[4] = {org[0] + i1, org[1] + i2, org[2] + i3, org[3] + i4};
       const bool row_ok = o[0] < p.odim[0] && o[1] < p.odim[1] && o[2] < p.odim[2] && o[3] < p.odim[3];
+      if (!row_ok) continue;
       const long long out_off = o[0] * p.ostride[0] + o[1] * p.ostride[1] + o[2] * p.ostride[2] + o[3] * p.ostride[3];
       const long long res_off = o[0] * p.rstride[0] + o[1] * p.rstride[1] + o[2] * p.rstride[2] + o[3] * p.rstride[3];
       const long long rv_off = (p.rowvec != nullptr)
                                    ? (o[0] * p.vstride[0] + o[1] * p.vstride[1] + o[2] * p.vstride[2] + o[3] * p.vstride[3])
                                    : 0;
-      const unsigned ok_mask = __ballot_sync(0xffffffffu, row_ok);
-      const int col_base = tn * ncols_out;  // first output column of this tile
-
-      if constexpr (EPI != EPI_GENERIC) {
-        // ---------------- specialised epilogues (see the header comment) ----------------
-        constexpr bool kGeglu = EPI == EPI_GEGLU;
-        constexpr bool kRes = EPI == EPI_RES;
-        constexpr int kColsOut = kGeglu ? BN / 2 : BN;  // output columns per tile
-        constexpr int kHalfCols = kColsOut / 2;         // contiguous share of each warp: 32 / 64 / 80 / 128 columns
-        const int c_begin = half_sel * kHalfCols;
-        const int c_end = c_begin + kHalfCols;
-        const int col0 = tn * kColsOut;
-        const bool has_bias = p.bias != nullptr;
-        auto unit_valid = [&](int u0) { return min(64, min(c_end - u0, p.n_out - (col0 + u0))); };  // multiple of 8
-        auto prefetch = [&](int u0) {
-          const int ucol = col0 + u0;
-          const int uvalid = unit_valid(u0);
+      if (geglu) {
+        // weight rows of tile tn: [value rows of BN/2 output columns][the matching gate rows]
 #pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rowi = it * 4 + rsub;
-            const long long roff = __shfl_sync(0xffffffffu, res_off, rowi);
-            uint8_t* dst = stg_res + rowi * kStageRowBytes + ((seg ^ (rowi & 7)) << 4);
-            if (((ok_mask >> rowi) & 1u) && seg * 8 < uvalid) cp_async_16(dst, p.residual + roff + ucol + seg * 8);
-            else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
+        for (int j = 0; j < BN / 16; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          const int col = tn * (BN / 2) + c;
+          if (col >= p.n_out) continue;  // n_out is a multiple of 8: both columns of the pair exist
+          float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+          float g0 = acc[4 * (j + BN / 16) + 2 * h], g1 = acc[4 * (j + BN / 16) + 2 * h + 1];
+          if (p.bias != nullptr) {
+            const float2 ba = __ldg(reinterpret_cast<const float2*>(p.bias + tn * BN + c));
+            const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + tn * BN + BN / 2 + c));
+            a0 += ba.x; a1 += ba.y; g0 += bg.x; g1 += bg.y;
           }
-        };
-        if (kRes && col0 + c_begin < p.n_out) prefetch(c_begin);  // overlaps the wait for this tile's MMAs
-
-        TR_WAIT(tr_wait_accfull, mbar_wait(&acc_full[acc], acc_phase));
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + acc * Cfg::kAccStride + (static_cast<uint32_t>(q * 32) << 16);
-
-        for (int u0 = c_begin; u0 < c_end; u0 += 64) {
-          const int ucol = col0 + u0;
-          if (ucol >= p.n_out) break;
-          const int uvalid = unit_valid(u0);
-          if (kRes) {
-            TR_WAIT(tr_wait_cp, cp_async_wait_all(); __syncwarp());
-          }
-#pragma unroll
-          for (int hsel = 0; hsel < 2; ++hsel) {
-            if (hsel * 32 >= uvalid) break;
-            const int c0 = u0 + hsel * 32;              // first column (inside the tile's output columns)
-            const int nvalid = uvalid - hsel * 32;      // >= 8, multiple of 8; groups of 8 beyond it do not exist
-            uint32_t va[32];
-            [[maybe_unused]] uint32_t vg[kGeglu ? 32 : 1];
-            tmem_ld_32x32(t_row + c0, va);
-            if constexpr (kGeglu) tmem_ld_32x32(t_row + BN / 2 + c0, vg);
-            // fp32 bias rows: value columns (and the matching gate rows for GEGLU); uniform addresses -> broadcast
-            const float4* bias_a = reinterpret_cast<const float4*>(p.bias + (kGeglu ? tn * BN + c0 : col0 + c0));
-            [[maybe_unused]] const float4* bias_g = reinterpret_cast<const float4*>(p.bias + tn * BN + BN / 2 + c0);
-            // every bias load of this 32-column slice is issued BEFORE waiting for the TMEM load: inside the per-8-column
-            // loop (behind its early exit) each group paid an exposed L1/L2 round trip, most of the epilogue's latency,
-            // which bounds the small-K GEMMs and the un-overlapped epilogue of every launch's last tile
-            // (round 2 A/B: 181.8 -> 174.9 ms / SDXL step, profiles/r2_experiments.md)
-            float4 bq[8];
-            [[maybe_unused]] float4 bqg[kGeglu ? 8 : 1];
-            if (has_bias) {
-#pragma unroll
-              for (int j8 = 0; j8 < 4; ++j8) {
-                if (j8 * 8 < nvalid) {
-                  bq[2 * j8] = __ldg(bias_a + j8 * 2);
-                  bq[2 * j8 + 1] = __ldg(bias_a + j8 * 2 + 1);
-                  if constexpr (kGeglu) {
-                    bqg[2 * j8] = __ldg(bias_g + j8 * 2);
-                    bqg[2 * j8 + 1] = __ldg(bias_g + j8 * 2 + 1);
-                  }
-                }
-              }
-            }
-            TR_WAIT(tr_tmem, tmem_ld_wait());
-#pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              if (j8 * 8 >= nvalid) break;
-              float x[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) x[e] = __uint_as_float(va[j8 * 8 + e]);
-              if (has_bias) {
-                const float4 b0 = bq[j8 * 2], b1 = bq[j8 * 2 + 1];
-                x[0] += b0.x; x[1] += b0.y; x[2] += b0.z; x[3] += b0.w;
-                x[4] += b1.x; x[5] += b1.y; x[6] += b1.z; x[7] += b1.w;
-              }
-              uint32_t w[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) w[e] = pack_bf16x2(x[2 * e], x[2 * e + 1]);  // bf16(acc + bias)
-              if constexpr (kGeglu) {
-                float g[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) g[e] = __uint_as_float(vg[j8 * 8 + e]);
-                if (has_bias) {
-                  const float4 b0 = bqg[j8 * 2], b1 = bqg[j8 * 2 + 1];
-                  g[0] += b0.x; g[1] += b0.y; g[2] += b0.z; g[3] += b0.w;
-                  g[4] += b1.x; g[5] += b1.y; g[6] += b1.z; g[7] += b1.w;
-                }
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const uint32_t gw = pack_bf16x2(g[2 * e], g[2 * e + 1]);             // bf16 gate
-                  const uint32_t lw = pack_bf16x2(gelu_erf(bf16lo_to_float(gw)), gelu_erf(bf16hi_to_float(gw)));
-                  w[e] = mul_bf16x2(w[e], lw);                                          // bf16(value * bf16 gelu)
-                }
-              }
-              if constexpr (kRes) {
-                const uint4 rr4 = *reinterpret_cast<const uint4*>(stg_res + lane * kStageRowBytes +
-                                                                  (((hsel * 4 + j8) ^ (lane & 7)) << 4));
-                w[0] = add_bf16x2(w[0], rr4.x); w[1] = add_bf16x2(w[1], rr4.y);
-                w[2] = add_bf16x2(w[2], rr4.z); w[3] = add_bf16x2(w[3], rr4.w);
-              }
-              *reinterpret_cast<uint4*>(stg_out + lane * kStageRowBytes + (((hsel * 4 + j8) ^ (lane & 7)) << 4)) =
-                  make_uint4(w[0], w[1], w[2], w[3]);
-            }
-          }
-          __syncwarp();  // staged rows complete; residual buffer fully consumed
-          if (kRes && u0 + 64 < c_end && col0 + u0 + 64 < p.n_out) prefetch(u0 + 64);
-          // ---- coalesced copy-out: 4 rows x 128 bytes per warp instruction ----
-          __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out);
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rowi = it * 4 + rsub;
-            const long long ooff = __shfl_sync(0xffffffffu, out_off, rowi);
-            if (((ok_mask >> rowi) & 1u) && seg * 8 < uvalid) {
-              const uint4 u = *reinterpret_cast<const uint4*>(stg_out + rowi * kStageRowBytes + ((seg ^ (rowi & 7)) << 4));
-              *reinterpret_cast<uint4*>(outp + ooff + ucol + seg * 8) = u;
-            }
-          }
-          __syncwarp();
+          round2_bf16(a0, a1);
+          round2_bf16(g0, g1);
+          float l0 = gelu_erf(g0), l1 = gelu_erf(g1);
+          round2_bf16(l0, l1);
+          float r0 = a0 * l0, r1 = a1 * l1;
+          round2_bf16(r0, r1);
+          gemm_finish_pair(p, r0, r1, col, 2, out_off, res_off, rv_off, alpha_s, alpha_t);
         }
       } else {
-        // asynchronous prefetch of the residual rows of one 64-column unit into stg_res (zero fill where invalid)
-        auto prefetch_res = [&](int u0) {
-          const int ucol = col_base + u0;
-          const int uvalid = min(64, min(ncols_out - u0, p.n_out - ucol));
-  #pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rowi = it * 4 + rsub;
-            const long long roff = __shfl_sync(0xffffffffu, res_off, rowi);
-            uint8_t* dst = stg_res + rowi * kStageRowBytes + ((seg ^ (rowi & 7)) << 4);
-            if (((ok_mask >> rowi) & 1u) && seg * 8 < uvalid) cp_async_16(dst, p.residual + roff + ucol + seg * 8);
-            else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * (lane & 3);
+          const int col = tn * BN + c;
+          if (col >= p.n_out) continue;
+          const int nv = min(2, p.n_out - col);
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.bias != nullptr) {
+            v0 += __ldg(p.bias + col);
+            v1 += __ldg(p.bias + min(col + 1, p.n_out - 1));
           }
-        };
-        const int u_first = half_sel * 64;
-        const bool has_units = u_first < ncols_out && col_base + u_first < p.n_out;
-        if (use_res && has_units) prefetch_res(u_first);  // overlaps the wait for this tile's MMAs
-
-        TR_WAIT(tr_wait_accfull, mbar_wait(&acc_full[acc], acc_phase));
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + acc * Cfg::kAccStride + (static_cast<uint32_t>(q * 32) << 16);
-
-        for (int u0 = u_first; u0 < ncols_out; u0 += 128) {
-          const int ucol = col_base + u0;          // first output column of this 64-wide unit
-          if (ucol >= p.n_out) break;
-          const int uvalid = min(64, min(ncols_out - u0, p.n_out - ucol));  // columns of the unit that exist
-          if (use_res) {
-            TR_WAIT(tr_wait_cp, cp_async_wait_all(); __syncwarp());
+          if (!p.out_fp32) round2_bf16(v0, v1);
+          if (p.act == CA_ACT_SILU) {
+            v0 = __fdividef(v0, 1.0f + __expf(-v0));
+            v1 = __fdividef(v1, 1.0f + __expf(-v1));
+            round2_bf16(v0, v1);
           }
-  #pragma unroll
-          for (int hsel = 0; hsel < 2; ++hsel) {
-            const int c0 = u0 + hsel * 32;      // column offset inside the tile's output columns
-            if (hsel * 32 >= uvalid) break;
-            const int col = col_base + c0;
-            const int nvalid = min(32, uvalid - hsel * 32);
-            uint32_t va[32];
-            tmem_ld_32x32(t_row + c0, va);
-            if (plain) {
-              // bias only: a single rounding straight into the staged row
-              TR_WAIT(tr_tmem, tmem_ld_wait());
-  #pragma unroll
-              for (int j8 = 0; j8 < 4; ++j8) {
-                float x[8];
-  #pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  x[e] = __uint_as_float(va[j8 * 8 + e]);
-                  if (p.bias != nullptr) x[e] += __ldg(p.bias + min(col + j8 * 8 + e, p.n_out - 1));
-                }
-                *reinterpret_cast<uint4*>(stg_out + lane * kStageRowBytes + (((hsel * 4 + j8) ^ (lane & 7)) << 4)) =
-                    make_uint4(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]), pack_bf16x2(x[4], x[5]),
-                               pack_bf16x2(x[6], x[7]));
-              }
-              continue;
-            }
-            float v[32];
-            if (geglu) {
-              uint32_t vg[32];
-              tmem_ld_32x32(t_row + BN / 2 + c0, vg);
-              TR_WAIT(tr_tmem, tmem_ld_wait());
-  #pragma unroll
-              for (int j = 0; j < 32; j += 2) {
-                const int wa = tn * BN + c0 + j;           // weight rows (value half)
-                const int wg = tn * BN + BN / 2 + c0 + j;  // weight rows (gate half)
-                float a0 = __uint_as_float(va[j]), a1 = __uint_as_float(va[j + 1]);
-                float g0 = __uint_as_float(vg[j]), g1 = __uint_as_float(vg[j + 1]);
-                if (p.bias != nullptr) {
-                  const float2 ba = __ldg(reinterpret_cast<const float2*>(p.bias + wa));
-                  const float2 bg = __ldg(reinterpret_cast<const float2*>(p.bias + wg));
-                  a0 += ba.x; a1 += ba.y; g0 += bg.x; g1 += bg.y;
-                }
-                round2_bf16(a0, a1);
-                round2_bf16(g0, g1);
-                float l0 = 0.5f * g0 * (1.0f + fast_erf(g0 * 0.70710678118654752440f));
-                float l1 = 0.5f * g1 * (1.0f + fast_erf(g1 * 0.70710678118654752440f));
-                round2_bf16(l0, l1);
-                float r0 = a0 * l0, r1 = a1 * l1;
-                round2_bf16(r0, r1);
-                v[j] = r0;
-                v[j + 1] = r1;
-              }
-            } else {
-              TR_WAIT(tr_tmem, tmem_ld_wait());
-  #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                float x = __uint_as_float(va[j]);
-                if (p.bias != nullptr) x += __ldg(p.bias + min(col + j, p.n_out - 1));
-                v[j] = x;
-              }
-              if (!p.out_fp32) {
-  #pragma unroll
-                for (int j = 0; j < 32; j += 2) round2_bf16(v[j], v[j + 1]);
-              }
-              if (p.act == CA_ACT_SILU) {
-  #pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                  v[j] = __fdividef(v[j], 1.0f + __expf(-v[j]));
-                  v[j + 1] = __fdividef(v[j + 1], 1.0f + __expf(-v[j + 1]));
-                  round2_bf16(v[j], v[j + 1]);
-                }
-              }
-            }
-            if (p.out_scale != 1.0f) {
-  #pragma unroll
-              for (int j = 0; j < 32; j += 2) {
-                v[j] *= p.out_scale;
-                v[j + 1] *= p.out_scale;
-                if (!p.out_fp32) round2_bf16(v[j], v[j + 1]);  // fp32 output (attention scores of the VAE): unrounded
-              }
-            }
-            if (p.rowvec != nullptr && row_ok) {
-              const __nv_bfloat16* rv = p.rowvec + rv_off + col;
-              if (nvalid == 32) {
-  #pragma unroll
-                for (int j8 = 0; j8 < 4; ++j8) {
-                  const uint4 u = __ldg(reinterpret_cast<const uint4*>(rv) + j8);
-                  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-  #pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float2 f = __bfloat1622float2(h[e]);
-                    v[j8 * 8 + e * 2] += f.x;
-                    v[j8 * 8 + e * 2 + 1] += f.y;
-                    round2_bf16(v[j8 * 8 + e * 2], v[j8 * 8 + e * 2 + 1]);
-                  }
-                }
-              } else {
-  #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                  if (j < nvalid) v[j] = round_bf16(v[j] + __bfloat162float(rv[j]));
-              }
-            }
-            if (p.out_fp32) {
-              // test / debug path: fp32 result, optional residual, direct stores
-              if (row_ok) {
-                float* op = reinterpret_cast<float*>(p.out) + out_off + col;
-  #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  if (j < nvalid) {
-                    float x = v[j];
-                    if (p.residual != nullptr) x += __bfloat162float(p.residual[res_off + col + j]);
-                    op[j] = x;
-                  }
-                }
-              }
-              continue;
-            }
-            if (use_res) {
-              // own row of the prefetched residual tile: 16-byte units hsel*4 .. hsel*4+3
-  #pragma unroll
-              for (int j8 = 0; j8 < 4; ++j8) {
-                const uint4 u = *reinterpret_cast<const uint4*>(stg_res + lane * kStageRowBytes + (((hsel * 4 + j8) ^ (lane & 7)) << 4));
-                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-  #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = __bfloat1622float2(h[e]);
-                  v[j8 * 8 + e * 2] += f.x;
-                  v[j8 * 8 + e * 2 + 1] += f.y;
-                  round2_bf16(v[j8 * 8 + e * 2], v[j8 * 8 + e * 2 + 1]);
-                }
-              }
-            }
-            if (p.blend_src != nullptr && row_ok) {
-              const __nv_bfloat16* bs = p.blend_src + res_off + col;
-  #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                if (j < nvalid) {
-                  const float xs = __bfloat162float(bs[j]);
-                  v[j] = round_bf16(round_bf16(alpha_s * xs) + round_bf16(alpha_t * v[j]));
-                }
-              }
-            }
-  #pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              *reinterpret_cast<uint4*>(stg_out + lane * kStageRowBytes + (((hsel * 4 + j8) ^ (lane & 7)) << 4)) =
-                  make_uint4(pack_bf16x2(v[j8 * 8 + 0], v[j8 * 8 + 1]), pack_bf16x2(v[j8 * 8 + 2], v[j8 * 8 + 3]),
-                             pack_bf16x2(v[j8 * 8 + 4], v[j8 * 8 + 5]), pack_bf16x2(v[j8 * 8 + 6], v[j8 * 8 + 7]));
-            }
-          }
-          if (!p.out_fp32) {
-            __syncwarp();  // staged rows complete; residual buffer fully consumed
-            const int u_next = u0 + 128;
-            if (use_res && u_next < ncols_out && col_base + u_next < p.n_out) prefetch_res(u_next);
-            // ---- coalesced copy-out: 4 rows x 128 bytes per warp instruction ----
-            __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(p.out);
-  #pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int rowi = it * 4 + rsub;
-              const long long ooff = __shfl_sync(0xffffffffu, out_off, rowi);
-              if (((ok_mask >> rowi) & 1u) && seg * 8 < uvalid) {
-                const uint4 u = *reinterpret_cast<const uint4*>(stg_out + rowi * kStageRowBytes + ((seg ^ (rowi & 7)) << 4));
-                *reinterpret_cast<uint4*>(outp + ooff + ucol + seg * 8) = u;
-              }
-            }
-            __syncwarp();
-          }
+          gemm_finish_pair(p, v0, v1, col, nv, out_off, res_off, rv_off, alpha_s, alpha_t);
         }
       }
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the (leader's) MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        TR_WAIT(tr_arrive, if (NCTA == 2) mbar_arrive_leader(&acc_empty[acc]); else mbar_arrive(&acc_empty[acc]));
-      }
-#ifdef CA_TRACE
-      ++tr_tiles;
-#endif
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-    if (lane == 0 && (ew == 0 || ew == 7)) {
-      [[maybe_unused]] const int o8 = (ew == 0) ? 0 : 5;  // two sampled epilogue warps: slots 4..7,9 and 10..14
-      TR_PUT(o8 == 0 ? 4 : 10, tr_wait_accfull);
-      TR_PUT(o8 == 0 ? 5 : 11, TR_NOW() - tr_start);
-      TR_PUT(o8 == 0 ? 6 : 12, tr_wait_cp);
-      TR_PUT(o8 == 0 ? 7 : 13, tr_arrive);
-      TR_PUT(o8 == 0 ? 9 : 14, tr_tiles);
-      if (ew == 0) TR_PUT(15, tr_tmem);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (NCTA == 2) cluster_sync_all();  // the peer may still signal this CTA's barriers / read its smem
-  if (warp == 2) {
-    tc_fence_after();
-    if (NCTA == 2) tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 
-template <int BN, int NCTA, int EPI>
-static cudaError_t launch_cfg(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, NCTA>;
+// one translation unit per BN (gemm_conv_bn*.cu) instantiates its kernel through this
+template <int BN>
+static cudaError_t launch_bn(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
+                             int grid, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
-  auto kern = gemm_conv_kernel<BN, NCTA, EPI>;
+  auto kern = gemm_conv_kernel<BN>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(Cfg::kSmemBytes));
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(grid));
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = NCTA;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-#ifndef CA_NO_PDL
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.numAttrs = 2;
-#endif
-  return cudaLaunchKernelEx(&cfg, kern, a0, a1, w, p);
-}
-
-// one translation unit per BN (gemm_conv_bn*.cu) instantiates its kernels through this
-template <int BN>
-static cudaError_t launch_bn(int ncta, int epi, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
-                             const GemmParams& p, int grid, cudaStream_t stream) {
-  if (ncta == 1) return launch_cfg<BN, 1, EPI_GENERIC>(a0, a1, w, p, grid, stream);  // A/B debugging only
-  switch (epi) {
-    case EPI_PLAIN: return launch_cfg<BN, 2, EPI_PLAIN>(a0, a1, w, p, grid, stream);
-    case EPI_RES: return launch_cfg<BN, 2, EPI_RES>(a0, a1, w, p, grid, stream);
-    case EPI_GEGLU:
-      if constexpr (BN == 256) return launch_cfg<BN, 2, EPI_GEGLU>(a0, a1, w, p, grid, stream);
-      else return launch_cfg<BN, 2, EPI_GENERIC>(a0, a1, w, p, grid, stream);
-    default: return launch_cfg<BN, 2, EPI_GENERIC>(a0, a1, w, p, grid, stream);
-  }
+  CA_KERNEL_LAUNCH(kern, grid, kGemmThreads, Cfg::kSmemBytes, stream, a0, a1, w, p);
+  return cudaGetLastError();
 }
 
 }  // namespace ca

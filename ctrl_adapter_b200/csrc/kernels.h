@@ -37,9 +37,7 @@ struct GemmParams {
   unsigned long long* trace;  // developer builds (-DCA_TRACE) only: per-CTA role wait-cycle counters, else unused
 };
 
-cudaError_t launch_gemm_wide(int epi, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                             int grid, cudaStream_t stream);
-cudaError_t launch_gemm_conv(int bn, int ncta, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
+cudaError_t launch_gemm_conv(int bn, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
                              const GemmParams& p, int grid, cudaStream_t stream);
 
 struct AttnParams {
@@ -50,9 +48,6 @@ struct AttnParams {
   float scale_log2;    // softmax scale * log2(e)
   __nv_bfloat16* out;  // [batch, lq, heads * 64 * v_slices]
   long long out_batch_stride, out_row_stride;  // elements
-  unsigned long long* trace;  // -DCA_TRACE builds only
-  unsigned backoff_ns;        // nanosleep per poll of the producer / MMA warps once a wait has lasted a few polls
-  unsigned stagger_ns;        // start offset between the two persistent CTAs of an SM (0 = none)
 };
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p,
                              cudaStream_t stream);

@@ -255,7 +255,7 @@ cudaError_t launch_gn_apply(const __nv_bfloat16* x0, int c0, const __nv_bfloat16
 //    no register cost.
 //  * The rows are NOT held in registers: both passes re-read their vectors from the stage.  The registers hold gamma
 //    and beta instead (16 x NV per lane; a lane's columns are the same for every row).  Loading them per row ran the
-//    kernel at the L1 rate: 8 bytes of fp32 gamma / beta per 2-byte element (profiles/r2_layernorm_ab.md).
+//    kernel at the L1 rate: 8 bytes of fp32 gamma / beta per 2-byte element.
 //  * Statistics in ONE pass over d = x - K with K = the row's first element: mean = K + sum(d)/C,
 //    var = (sum(d^2) - sum(d)^2 / C) / C.  K is an element of the row, so (K - mean)^2 <= (C - 1) var and the
 //    cancellation costs at most ~C ulp of fp32 in var (1.5e-4 relative at C = 1280), far below the bf16 output grid.

@@ -1,211 +1,143 @@
 // Temporal self-attention of the video adapters / UNets on the tensor cores: the sequence is the F <= 32 frames of one
-// pixel (head dim 64), so one (pixel, head) problem is a 16 x 16 (or 32 x 32) score matrix -- far below a tcgen05 tile.
+// pixel (head dim 64), so one (pixel, head) problem is a 16 x 16 (or 32 x 32) score matrix -- far below a wgmma tile.
 // A CTA therefore batches G = 128 / SEQ pixels of one (clip, head) into ONE 128-row tile:
 //
 //   TMA: the tensor map orders the global dims as (channel, FRAME, PIXEL, clip) -- strides are free, so the box
 //        (64, SEQ, G, 1) lands in shared memory as rows (pixel g, frame f): each pixel's sequence is a contiguous block of
 //        SEQ rows (frames >= F and pixels >= hw are zero-filled by the TMA unit).
-//   MMA: S = Q K^T as one M128 N128 K64 tcgen05.mma; only the G diagonal SEQ x SEQ blocks are meaningful (the other
-//        blocks cost tensor cycles the kernel has to spare: it is HBM-bound, 64 KB of traffic per tile).
-//   softmax: thread r owns row r and reads the 32 columns that contain its diagonal block (one tcgen05.ld), masks the
-//        rest, exponentiates, writes bf16 P into the diagonal strip of a [128 x 128] shared-memory tile whose
-//        off-diagonal part stays zero from the kernel prologue.
-//   MMA: O = P V (M128 N64 K128, V consumed MN-major exactly as in attention.cu), epilogue O / l -> global.
-//
-// Replaces round 1's FMA kernel (one warp per (pixel, head), 0.96 TB/s = 0.15 of the HBM peak, instruction-bound:
-// ~2200 instructions per 6 KB).  Same rounding points: fp32 scores and row sum, P rounded to bf16 before PV, one bf16
-// rounding of O / l.
-// Roles (256 threads, one CTA per SM, persistent over tiles): warp 0 = TMA producer (3-stage ring of Q/K/V tiles),
-// warp 1 = MMA issuer + TMEM allocator, warps 4-7 = softmax + epilogue.
+//   MMA: SEQ divides 64, so no sequence straddles a 64-row half.  For each half, S = Q K^T as one m64n64k64 wgmma; only
+//        the diagonal SEQ x SEQ blocks are meaningful, the others are masked.
+//   softmax in registers (fp32 scores and row sum, P rounded to bf16), then O = P V as m64n64k64 with P from registers
+//        and V read MN-major from shared memory; epilogue O / l -> global.
+// One warpgroup per CTA (128 threads, 48 KB of shared memory), so several CTAs share an SM and one CTA's loads overlap
+// another's MMAs.
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace ca {
 
-static constexpr int kTaThreads = 256;
-static constexpr int kTaStages = 3;
-static constexpr uint32_t kTaTile = 128 * 64 * 2;               // one [128 rows x 64 dims] bf16 tile = 16 KB
-static constexpr uint32_t kTaStageBytes = 3 * kTaTile;          // Q, K, V
-static constexpr uint32_t kTaPBytes = 2 * kTaTile;              // P [128 x 128] bf16 as two 64-key swizzle chunks
-static constexpr uint32_t kTaSmem = kTaStages * kTaStageBytes + kTaPBytes + 1024;
+static constexpr int kTaThreads = 128;
+static constexpr uint32_t kTaTile = 128 * 64 * 2;  // one [128 rows x 64 dims] bf16 tile = 16 KB
+static constexpr uint32_t kTaSmem = 3 * kTaTile + 1024 /*align slack*/ + 64 /*barrier*/;
 
 template <int SEQ>
-__global__ void __launch_bounds__(kTaThreads, 1)
+__global__ void __launch_bounds__(kTaThreads)
 temporal_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                              const __grid_constant__ CUtensorMap tmap_v, const TemporalAttnParams p) {
   constexpr int G = 128 / SEQ;  // pixels per tile
   CA_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
-  uint8_t* smem = smem_raw + pad;
-  uint8_t* smem_p = smem + kTaStages * kTaStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_p + kTaPBytes);
-  if (pad + kTaStages * kTaStageBytes + kTaPBytes + 128 > kTaSmem) __trap();
-  uint64_t* full = bars;             // [3]
-  uint64_t* empty = bars + 3;        // [3]
-  uint64_t* s_full = bars + 6;
-  uint64_t* p_full = bars + 7;
-  uint64_t* o_full = bars + 8;
-  uint64_t* o_free = bars + 9;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 3 * kTaTile);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int tig = lane & 3;
   const int ngroups = static_cast<int>((p.hw + G - 1) / G);
-  const long long total = static_cast<long long>(p.clips) * ngroups * p.heads;
-  auto decode = [&](long long w, int& head, int& pix0, int& clip) {
-    head = static_cast<int>(w % p.heads);
-    const long long t = w / p.heads;
-    pix0 = static_cast<int>(t % ngroups) * G;
-    clip = static_cast<int>(t / ngroups);
-  };
+  const long long w = blockIdx.x;
+  const int head = static_cast<int>(w % p.heads);
+  const long long t = w / p.heads;
+  const int pix0 = static_cast<int>(t % ngroups) * G;
+  const int clip = static_cast<int>(t / ngroups);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
-    for (int s = 0; s < kTaStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
-    mbar_init(o_free, 4);
+    mbar_init(bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<256>(tmem_slot);
-  // off-diagonal blocks of P are never written again: zero the whole tile once
-  for (uint32_t i = threadIdx.x; i < kTaPBytes / 16; i += kTaThreads) reinterpret_cast<uint4*>(smem_p)[i] = make_uint4(0, 0, 0, 0);
-  fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = *tmem_slot;
-  const uint32_t tmem_o = tmem_s + 128;
   CA_PDL_WAIT();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (long long w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        int head, pix0, clip;
-        decode(w, head, pix0, clip);
-        const int st = it % kTaStages;
-        mbar_wait(&empty[st], ((it / kTaStages) & 1) ^ 1);
-        uint8_t* dst = smem + st * kTaStageBytes;
-        mbar_arrive_expect_tx(&full[st], kTaStageBytes);
-        tma_load_4d(dst, &tmap_q, &full[st], head * 64, 0, pix0, clip);
-        tma_load_4d(dst + kTaTile, &tmap_k, &full[st], head * 64, 0, pix0, clip);
-        tma_load_4d(dst + 2 * kTaTile, &tmap_v, &full[st], head * 64, 0, pix0, clip);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64, 0, 1);  // B (= V tile) is MN-major
-      const uint32_t p_addr = smem_u32(smem_p);
-      uint32_t it = 0;
-      for (long long w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-        const int st = it % kTaStages;
-        const uint32_t base = smem_u32(smem + st * kTaStageBytes);
-        mbar_wait(&full[st], (it / kTaStages) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = umma_smem_desc_sw128(base + k * 32, 16, 1024);
-          const uint64_t db = umma_smem_desc_sw128(base + kTaTile + k * 32, 16, 1024);
-          umma_bf16_ss(tmem_s, da, db, idesc_s, k != 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        mbar_wait(p_full, it & 1);                 // P staged in shared memory (and fenced for the async proxy)
-        if (it > 0) mbar_wait(o_free, (it - 1) & 1);  // the previous tile's output has been read out of O
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t da = umma_smem_desc_sw128(p_addr + (k >> 2) * kTaTile + (k & 3) * 32, 16, 1024);
-          const uint64_t db = umma_smem_desc_sw128(base + 2 * kTaTile + k * 2048, 8192, 1024);
-          umma_bf16_ss(tmem_o, da, db, idesc_o, k != 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(&empty[st]);  // Q, K, V of this stage are no longer read once the PV MMAs retired
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const uint32_t lane_sel = static_cast<uint32_t>(q * 32) << 16;
-    const int f = r % SEQ, g = r / SEQ;
-    const int blk = lane / SEQ;  // which of the (32 / SEQ) sequences inside this warp's 32 columns is mine
-    uint8_t* p_row = smem_p + (q >> 1) * kTaTile + r * 128;
-    const int sw = r & 7;
-    uint32_t it = 0;
-    for (long long w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-      int head, pix0, clip;
-      decode(w, head, pix0, clip);
-      mbar_wait(s_full, it & 1);
-      tc_fence_after();
-      uint32_t sv[32];
-      tmem_ld_32x32(tmem_s + lane_sel + q * 32, sv);  // the 32 columns holding this row's diagonal block
-      tmem_ld_wait();
-      float mx = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const bool valid = (j / SEQ == blk) && (j % SEQ) < p.frames;
-        const float x = valid ? __uint_as_float(sv[j]) * p.scale_log2 : -INFINITY;
-        sv[j] = __float_as_uint(x);
-        mx = fmaxf(mx, x);
-      }
-      float l = 0.f;
-      uint32_t pw[16];
-#pragma unroll
-      for (int j = 0; j < 32; j += 2) {
-        const float p0 = exp2f(__uint_as_float(sv[j]) - mx), p1 = exp2f(__uint_as_float(sv[j + 1]) - mx);
-        l += p0 + p1;
-        pw[j >> 1] = pack_bf16x2(p0, p1);  // P is bf16 in the fused SDPA kernels of the reference path
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int unit = (q & 1) * 4 + u;  // 16-byte unit inside the 128-byte row of this 64-key chunk
-        *reinterpret_cast<uint4*>(p_row + ((unit ^ sw) << 4)) = make_uint4(pw[u * 4], pw[u * 4 + 1], pw[u * 4 + 2], pw[u * 4 + 3]);
-      }
-      fence_proxy_async_smem();  // P stores -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // epilogue
-      mbar_wait(o_full, it & 1);
-      tc_fence_after();
-      const float inv_l = 1.0f / l;
-      const long long pix = static_cast<long long>(pix0) + g;
-      const bool live = f < p.frames && pix < p.hw;
-      __nv_bfloat16* orow = p.out + ((static_cast<long long>(clip) * p.frames + f) * p.hw + pix) * p.out_row_stride + head * 64;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t ov[32];
-        tmem_ld_32x32(tmem_o + lane_sel + c * 32, ov);
-        tmem_ld_wait();
-        if (live) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = __uint_as_float(ov[u * 8 + e]) * inv_l;
-            *reinterpret_cast<uint4*>(orow + c * 32 + u * 8) = make_uint4(
-                pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_free);
-    }
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(bar, 3 * kTaTile);
+    tma_load_4d(smem, &tmap_q, bar, head * 64, 0, pix0, clip);
+    tma_load_4d(smem + kTaTile, &tmap_k, bar, head * 64, 0, pix0, clip);
+    tma_load_4d(smem + 2 * kTaTile, &tmap_v, bar, head * 64, 0, pix0, clip);
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_s);
+  mbar_wait(bar, 0);
+  const uint32_t base = smem_u32(smem);
+
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    const uint32_t off = half * 64 * 128;  // rows [64 half, 64 half + 64)
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      Wgmma<64>::ss(s, gmma_desc_sw128(base + off + k * 32, 16, 1024),
+                    gmma_desc_sw128(base + kTaTile + off + k * 32, 16, 1024), k != 0 ? 1 : 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+
+    // thread holds rows (r, r + 8) of this half x key columns 8 jj + 2 tig + {0, 1}
+    const int r_lo = warp * 16 + (lane >> 2);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int row = r_lo + 8 * (e >> 1);
+        const int col = 8 * jj + 2 * tig + (e & 1);
+        const bool valid = (col / SEQ == row / SEQ) && (col % SEQ) < p.frames;
+        const float x = valid ? s[4 * jj + e] * p.scale_log2 : -INFINITY;
+        s[4 * jj + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+    float l[2] = {0.f, 0.f};
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float pv = exp2f(s[i] - mx[(i >> 1) & 1]);
+      s[i] = pv;
+      l[(i >> 1) & 1] += pv;
+    }
+    uint32_t pa[4][4];  // P is bf16 in the fused SDPA kernels of the reference path
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      Wgmma<64>::rs_bt(o, pa[kk], gmma_desc_sw128(base + 2 * kTaTile + off + kk * 2048, 8192, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float lt = l[hh];
+      lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+      lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+      const float inv_l = 1.0f / lt;
+      const int row = half * 64 + r_lo + 8 * hh;  // tile row = g * SEQ + f
+      const int f = row % SEQ;
+      const long long pix = static_cast<long long>(pix0) + row / SEQ;
+      if (f >= p.frames || pix >= p.hw) continue;
+      __nv_bfloat16* orow =
+          p.out + ((static_cast<long long>(clip) * p.frames + f) * p.hw + pix) * p.out_row_stride + head * 64;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * tig) =
+            pack_bf16x2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
+      }
+    }
   }
 }
 
@@ -213,24 +145,16 @@ template <int SEQ>
 static cudaError_t launch_seq(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v,
                               const TemporalAttnParams& p, cudaStream_t stream) {
   static bool attr_set = false;
+  auto kern = temporal_attention_tc_kernel<SEQ>;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(temporal_attention_tc_kernel<SEQ>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(kTaSmem));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kTaSmem));
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) sms = 148;
-  }
   const long long groups = (p.hw + 128 / SEQ - 1) / (128 / SEQ);
   const long long total = static_cast<long long>(p.clips) * groups * p.heads;
-  if (total <= 0) return cudaErrorInvalidValue;
-  const int grid = static_cast<int>(total < sms ? total : sms);
-  auto kern = temporal_attention_tc_kernel<SEQ>;
-  CA_KERNEL_LAUNCH(kern, grid, kTaThreads, kTaSmem, stream, q, k, v, p);
+  if (total <= 0 || total > 0x7fffffffLL) return cudaErrorInvalidValue;
+  CA_KERNEL_LAUNCH(kern, static_cast<unsigned>(total), kTaThreads, kTaSmem, stream, q, k, v, p);
   return cudaGetLastError();
 }
 

@@ -1,8 +1,8 @@
-"""Host-side building blocks of the B200 hot path.
+"""Host-side building blocks of the H100 hot path.
 
 Each class is an ``nn.Module`` used ONLY as a parameter container with the reference's / diffusers' parameter names
 (so reference checkpoints load with ``load_state_dict``); ``forward`` never calls a PyTorch op on activations -- it
-launches the sm_100a kernels of ``csrc/`` through ``ops``.  Activations are channels-last bf16.
+launches the sm_90a kernels of ``csrc/`` through ``ops``.  Activations are channels-last bf16.
 
 Weights are repacked once (``pack()``, lazily on first use / after ``.to()``) into the kernel layouts:
 conv weights ``[Cout, taps*Cin]``, fused QKV / KV projection matrices, GEGLU rows interleaved per 256-wide N tile,

@@ -1,6 +1,6 @@
 """Torch-tensor front end of the C ABI: builds the descriptors (boxes, taps, strides) and launches on the
 current CUDA stream.  PyTorch is used only for device memory and streams; every computation below runs in
-the hand-written sm_100a kernels of ``csrc/`` (no fallback path).
+the hand-written sm_90a kernels of ``csrc/`` (no fallback path).
 
 Layouts: activations are channels-last, ``[N, H, W, C]`` / ``[tokens, C]`` bf16 contiguous.
 """

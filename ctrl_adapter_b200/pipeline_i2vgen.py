@@ -1,5 +1,5 @@
 """The I2VGen-XL denoising hot loop (body of /root/reference/i2vgen_xl/pipelines/i2vgen_xl_controlnet_adapter_pipeline.py
-:902-1118) on the B200 modules:
+:902-1118) on the H100 modules:
 
   ControlNet (or E ControlNets -> router -> weighted merge) -> Ctrl-Adapter (spatial + temporal) -> I2VGen-XL UNet with
   residual injection -> CFG -> DDIM update.

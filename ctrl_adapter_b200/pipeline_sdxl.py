@@ -1,5 +1,5 @@
 """The SDXL denoising hot loop (body of /root/reference/sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1279-1404)
-on the B200 modules:  [pool] -> ControlNet -> Ctrl-Adapter -> SDXL UNet (+ residual injection) -> CFG -> Euler step.
+on the H100 modules:  [pool] -> ControlNet -> Ctrl-Adapter -> SDXL UNet (+ residual injection) -> CFG -> Euler step.
 
 Everything outside the loop (prompt / image encoding, VAE) is out of scope (SURVEY.md section 8); the loop takes the
 already-encoded conditioning tensors.  ``step()`` is the plain public-API path (module ``forward`` calls);

@@ -1,5 +1,5 @@
 """The Stable-Video-Diffusion denoising hot loop (body of
-/root/reference/svd/pipelines/svd_controlnet_adapter_pipeline.py:640-787) on the B200 modules:
+/root/reference/svd/pipelines/svd_controlnet_adapter_pipeline.py:640-787) on the H100 modules:
 
   [pool to 64x64] -> ControlNet (timestep from the step index) -> [sparse key-frame gather] -> Ctrl-Adapter (spatial +
   temporal) -> [scatter] -> SVD UNet on cat(latents, image latents) with 5-D residual injection -> per-frame CFG ->
@@ -8,8 +8,7 @@
 Latents live in the reference's own (clip, frame, channel, h, w) order.  Per-step scalars sit in device rows so one
 captured CUDA graph serves every step.
 
-GPU parity: tests/test_video_paths_gpu.py groups `svd`, `svd_loop` (first green hardware run: round 2,
-profiles/r2_parity.md); CPU: the op-layer emulation against the restated reference loop.
+GPU parity: tests/test_video_paths_gpu.py groups `svd`, `svd_loop`; CPU: the op-layer emulation against the restated reference loop.
 """
 from __future__ import annotations
 

@@ -6,14 +6,14 @@ and with the reference's ``__init__`` / ``__call__`` signatures:
     svd.pipelines.svd_controlnet_adapter_pipeline.SVDControlNetAdapterPipeline                (:361-802)
 
 What runs here is the denoising loop -- the hot path (SURVEY.md section 8): the loop classes of pipeline_sdxl /
-pipeline_i2vgen / pipeline_svd on the B200 modules, CUDA-graph replayed.  Everything either side of the loop is a
+pipeline_i2vgen / pipeline_svd on the H100 modules, CUDA-graph replayed.  Everything either side of the loop is a
 different subsystem of the reference stack (CLIP text / vision encoders, the SD1.5 prompt helper, the VAE; SURVEY.md
 section 8f) and is *duck-typed*: a pipeline uses whatever ``text_encoder`` / ``helper`` / ``image_encoder`` / ``vae``
 objects it was constructed with (e.g. the diffusers / transformers ones where those libraries exist), and when one is
 absent the caller passes that stage's OUTPUT instead -- ``prompt_embeds`` ... exactly as the reference signature already
 allows, plus the keyword-only extensions listed in each ``__call__`` (``controlnet_prompt_embeds``, ``image_embeddings``,
 ``image_latents``, tensor ``control_images``).  ``output_type="latent"`` needs no VAE; with
-``vae=ctrl_adapter_b200.vae.AutoencoderKL`` the SDXL and I2VGen-XL pipelines decode on the B200 kernels as well.  Nothing
+``vae=ctrl_adapter_b200.vae.AutoencoderKL`` the SDXL and I2VGen-XL pipelines decode on the H100 kernels as well.  Nothing
 here falls back to a PyTorch implementation of the hot path.
 """
 from __future__ import annotations
@@ -57,7 +57,7 @@ class DiffusionPipeline:
     """The slice of diffusers' DiffusionPipeline the three pipelines use (SURVEY.md section 8b row 1): module registry,
     ``to()``, ``_execution_device``, ``progress_bar``, ``from_pretrained`` with component overrides."""
 
-    _unet_class = None      # set by the subclasses: the B200 UNet of the backbone
+    _unet_class = None      # set by the subclasses: the H100 UNet of the backbone
     _unet_subfolder = "unet"
 
     def __init__(self):
@@ -130,7 +130,7 @@ class DiffusionPipeline:
 # ------------------------------------------------------------------------------------------------------------------
 def _need(value, what: str, stage: str):
     if value is None:
-        raise ValueError(f"{what} is required: this pipeline has no {stage} (the encoder stages are outside the B200 hot "
+        raise ValueError(f"{what} is required: this pipeline has no {stage} (the encoder stages are outside the H100 hot "
                          f"path) -- pass the pre-encoded tensor")
     return value
 

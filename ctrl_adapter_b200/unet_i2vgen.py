@@ -1,4 +1,4 @@
-"""B200 host mirror of ``I2VGenXLUNet`` (/root/reference/i2vgen_xl/models/unets/unet_i2vgen_xl.py:104-761, a diffusers
+"""H100 host mirror of ``I2VGenXLUNet`` (/root/reference/i2vgen_xl/models/unets/unet_i2vgen_xl.py:104-761, a diffusers
 v0.27.2 copy with ``down_block_additional_residuals`` / ``mid_block_additional_residual`` added at :681-695, :709-714).
 
 Same constructor defaults, forward signature and state-dict keys.  Video activations are ``[B*F, H, W, C]`` bf16 in

@@ -1,4 +1,4 @@
-"""B200 host mirror of the SDXL ``UNet2DConditionModel`` (stock diffusers class in the reference: instantiated at
+"""H100 host mirror of the SDXL ``UNet2DConditionModel`` (stock diffusers class in the reference: instantiated at
 /root/reference/inference.py:369, called at sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1356-1366 with the
 adapter's ``down_block_additional_residuals`` and ``mid_block_additional_residual=0``).
 

@@ -1,4 +1,4 @@
-"""B200 host mirror of the Stable-Video-Diffusion UNet with the reference's residual injection
+"""H100 host mirror of the Stable-Video-Diffusion UNet with the reference's residual injection
 (/root/reference/svd/models/unets/unet_spatio_temporal_condition.py: constructor :71-245, forward :357-526, injection
 :457-471 and :485-490; instantiated at inference.py:360, called at svd/pipelines/svd_controlnet_adapter_pipeline.py).
 

@@ -1,4 +1,4 @@
-"""B200 host mirror of the decoder half of diffusers' ``AutoencoderKL`` -- the VAE ``decode`` the reference pipelines
+"""H100 host mirror of the decoder half of diffusers' ``AutoencoderKL`` -- the VAE ``decode`` the reference pipelines
 call after the denoising loop (/root/reference/sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1414;
 i2vgen_xl/pipelines/i2vgen_xl_controlnet_adapter_pipeline.py:398-418 ``decode_latents``; SURVEY.md section 8f row 1).
 

@@ -1,5 +1,5 @@
 /*
- * ctrl_adapter_b200 -- C ABI of the B200 (sm_100a) denoising hot path of Ctrl-Adapter.
+ * ctrl_adapter_b200 -- C ABI of the H100 (sm_90a) denoising hot path of Ctrl-Adapter.
  *
  * The reference (HL-hanlin/Ctrl-Adapter @ 4f495bd) has no FFI layer: its hot path is eager
  * PyTorch/diffusers `nn.Module.forward` calls (SURVEY.md section 8b).  This header is the boundary a
@@ -36,7 +36,7 @@ const char* ca_last_error(void);
 int ca_device_ok(void);
 
 /*
- * ca_gemm -- multi-tap tensor-core contraction (tcgen05) with fused epilogue.
+ * ca_gemm -- multi-tap tensor-core contraction (wgmma) with fused epilogue.
  *
  *   out[row, n] = epi( sum_tap sum_src sum_c  A_src[row + tap_off[tap], c] * W[n, tap, src, c] )
  *
@@ -94,7 +94,7 @@ typedef struct ca_gemm_desc {
 int ca_gemm(const ca_gemm_desc* d, void* cuda_stream);
 
 /*
- * ca_attention -- softmax(Q K^T * scale) V, flash-style, tcgen05 + TMA.
+ * ca_attention -- softmax(Q K^T * scale) V, flash-style, wgmma + TMA.
  * Replaces F.scaled_dot_product_attention (diffusers AttnProcessor2_0) reached from
  * model/adapter_spatial_temporal.py:271 (adapter spatial self / cross attention), the ControlNet
  * Transformer2DModel blocks built at controlnet/controlnet.py:371-424 and the UNet attention layers.

@@ -2,7 +2,7 @@
 our loop (bf16 kernels, CUDA-graph replay), the oracle as the reference runs it (eager bf16 autocast) and the oracle in
 fp32 (the truth) -- with the relative Frobenius distance to the truth after every step.
 
-  python scripts/drift_report.py sdxl|i2vgen|svd [--steps N] [--guidance-end E] --out gpurun_out/r2_drift_<w>.json
+  python scripts/drift_report.py sdxl|i2vgen|svd [--steps N] [--guidance-end E] --out drift_<w>.json
 
 sdxl: B=1 at 1024x1024 (50 steps);  i2vgen: B=1, F=16, 64x64 latents (config 3's clip geometry, 50 steps);
 svd: B=1, F=14, 32x32 latents, use_size_512=False (25 steps).  Oracle = test infrastructure (tests/module_checks.py builds

@@ -1,8 +1,7 @@
 """Aggregates an ncu launch list (`--metrics gpu__time_duration.sum[,dram__bytes_read.sum,dram__bytes_write.sum] --csv`)
 per kernel: launches, total time, share and (when captured) average DRAM bytes per launch.
-usage: python scripts/launch_share.py gpurun_out/launches.csv [skip_launches] [traffic.json] > profiles/<round>_launch_shares.md
-The optional third argument writes {kernel base name: {"launches", "dram_bytes_per_launch"}} for bench.py's
-roofline.traffic field.
+usage: python scripts/launch_share.py launches.csv [skip_launches] [traffic.json] > launch_shares.md
+The optional third argument writes {kernel base name: {"launches", "dram_bytes_per_launch"}}.
 
 The per-launch times of such a pass are cold-cache and serialised, so only the SHARE of each kernel is meaningful; the
 absolute step time comes from bench.py's CUDA events."""

@@ -1,4 +1,4 @@
-"""Summarises .ncu-rep captures (read here, on the GPU-less box) into profiles/<name>.md tables."""
+"""Summarises .ncu-rep captures into markdown tables (runs without a GPU)."""
 import csv
 import subprocess
 import sys

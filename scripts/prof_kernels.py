@@ -60,7 +60,7 @@ elif which.startswith("tattn"):  # temporal attention at config 3's adapter-A sh
     nbytes = 4.0 * clips * frames * hw * inner * 2
 elif which in ("ln", "ln640", "ln320"):
     rows, c = {"ln": (16384, 1280), "ln640": (65536, 640), "ln320": (131072, 320)}[which]
-    xs = [rnd(rows, c) for _ in range(8)]   # 8 x 42 MB rotate through the 126 MB L2: every launch reads from HBM
+    xs = [rnd(rows, c) for _ in range(8)]   # 8 x 42 MB rotate through the 50 MB L2: every launch reads from HBM
     g, b = torch.ones(c, device=dev), torch.zeros(c, device=dev)
     _i = [0]
 

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box with -m gpu)")
     config.addinivalue_line("markers", "slow: multi-minute CPU test (full-width 1.5-2.6 B parameter UNets through the ops "
                                        "emulator); skipped unless CA_RUN_SLOW=1")
 

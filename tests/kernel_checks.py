@@ -94,12 +94,23 @@ def check_geglu(m, k, d, seed=0):
     x = _rand(m, k, seed=seed + 1)
     w = _rand(2 * d, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
     b = _rand(2 * d, seed=seed + 3)
-    h = (x.float() @ w.float().t() + b.float()).to(BF16).float()
-    a, g = h[:, :d], h[:, d:]
-    ref = (a * F.gelu(g).to(BF16).float()).to(BF16).float()
     wi, bi = ops.pack_geglu_weight(w, b, 256)
     out = ops.linear(x, wi, ops.bias_f32(bi), act=ops.ACT_GEGLU, bn=256)
+    # the same contraction (same kernel, tiles and summation order) with the fp32 pre-activation as output
+    pre = ops.linear(x, wi, ops.bias_f32(bi), out_fp32=True, bn=256).reshape(m, d // 128, 2, 128)
+    pre = torch.cat([pre[:, :, 0].reshape(m, d), pre[:, :, 1].reshape(m, d)], dim=1)  # undo the per-tile interleave
     torch.cuda.synchronize()
+    # (1) the contraction against the exact (fp64) pre-activation at the fp32 GEMM tolerance of check_linear
+    exact = (x.double() @ w.double().t() + b.double()).float()
+    _report(f"geglu pre-activation m{m} k{k} d{2 * d}", pre, exact, 1e-3, 1e-4)
+    # (2) the epilogue's bf16 rounding chain applied to the pre-activation the kernel accumulated.  A pre-activation
+    # within an fp32 ulp or two of a bf16 rounding tie rounds either way depending on the summation order (cuBLAS's
+    # own fp32 result rounds ~3300 of the 25.6 M pre-activations at m5000 away from the exact value), and GELU times
+    # the value half magnifies that one-ulp flip beyond the output tolerance, so the epilogue is checked against the
+    # input it was given.
+    h = pre.to(BF16).float()
+    a, g = h[:, :d], h[:, d:]
+    ref = (a * F.gelu(g).to(BF16).float()).to(BF16).float()
     return _report(f"geglu m{m} k{k} d{d}", out, ref, 2 ** -6, 2e-3)
 
 
@@ -122,11 +133,13 @@ def check_linear_blend(m, k, n, seed=0):
     res = _rand(m, n, seed=seed + 4)
     xs = _rand(m, n, seed=seed + 5)
     alpha = torch.sigmoid(torch.tensor([0.3], device="cuda")).to(BF16)
-    xt = ((x.float() @ w.float().t()).to(BF16).float() + res.float()).to(BF16)
+    lin = (x.float() @ w.float().t()).to(BF16).float()
+    xt = (lin + res.float()).to(BF16)
     ref = ((alpha * xs).to(BF16) + ((1.0 - alpha).to(BF16) * xt).to(BF16)).float()
     out = ops.linear(x, w, None, residual=res, blend_src=xs, blend_alpha=alpha.float())
     torch.cuda.synchronize()
     mag = torch.maximum(torch.maximum(xt.float().abs(), res.float().abs()), xs.float().abs())
+    mag = torch.maximum(mag, lin.abs())  # bf16(x @ w^T) is the first rounded intermediate of the epilogue
     return _report(f"linear+res+blend m{m} k{k} n{n}", out, ref, 2 ** -7, 1e-3, mag=mag)
 
 

@@ -1,4 +1,4 @@
-"""GPU parity checks at module level: the B200 modules (ctrl_adapter_b200.*) against the oracle on identical
+"""GPU parity checks at module level: the H100 modules (ctrl_adapter_b200.*) against the oracle on identical
 name-seeded weights and inputs.
 
 Comparison point (SURVEY.md "hard parts"): the ground truth is the oracle in fp32 (TF32 off) evaluated with the SAME

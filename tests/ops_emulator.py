@@ -5,7 +5,7 @@ Purpose: the host modules (layers / adapter / controlnet / unet_*) are pure comp
 emulator patched in, that logic -- block wiring, skip / residual order, strides, per-clip broadcast rows, weight packing
 -- is checked against the oracle on the CPU box (`tests/test_host_emulated_cpu.py`), where there is no GPU.  It is never
 imported by the product (the product has no CPU path and fails loudly without the CUDA library); the numerics of the
-kernels themselves are checked on the B200 by tests/kernel_checks.py.
+kernels themselves are checked on the H100 by tests/kernel_checks.py.
 """
 from __future__ import annotations
 

@@ -5,7 +5,7 @@ modules are compared with the oracle on identical name-seeded, bf16-quantised we
 What this pins without a GPU: block wiring, skip / residual order (zip truncation), weight packing (conv taps, fused QKV,
 GEGLU tile interleave, padded heads), per-image / per-clip broadcast rows, the single-token cross-attention collapse and
 the reference quirks that live in host code (e.g. the (pixel, clip) ordering of `time_context`).  Kernel numerics are a
-separate matter (tests/kernel_checks.py on the B200).  Tolerance: the emulation rounds to bf16 where the kernels do, the
+separate matter (tests/kernel_checks.py on the H100).  Tolerance: the emulation rounds to bf16 where the kernels do, the
 oracle runs in fp32 -> relative Frobenius error at the bf16 level (<= 3e-2), the same bar as the GPU module checks.
 """
 import pytest

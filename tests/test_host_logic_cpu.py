@@ -192,7 +192,7 @@ def test_pretrained_folder_roundtrip(tmp_path):
 
 
 def test_reference_import_paths_resolve():
-    """SURVEY.md section 8b: the module paths AND NAMES inference.py imports (:351-367) exist and resolve to the B200-backed
+    """SURVEY.md section 8b: the module paths AND NAMES inference.py imports (:351-367) exist and resolve to the H100-backed
     classes (or, for the out-of-scope helpers, to stubs that fail loudly when used)."""
     import argparse
     from controlnet.controlnet import ControlNetModel  # noqa: F401

@@ -1,4 +1,4 @@
-"""pytest -m gpu: the B200 modules (ControlNetAdapter, ControlNetRouter, ControlNetModel, SDXL UNet2DConditionModel)
+"""pytest -m gpu: the H100 modules (ControlNetAdapter, ControlNetRouter, ControlNetModel, SDXL UNet2DConditionModel)
 against the oracle on identical name-seeded weights/inputs (tolerances: tests/module_checks.py header)."""
 import pytest
 import torch

@@ -1,8 +1,7 @@
 """pytest -m gpu: Stable-Video-Diffusion UNet, the SVD denoising loop (ca_cfg_euler_v), the sparse key-frame path of the
 I2VGen-XL loop, the SVD-geometry kernel shapes and the folded conditioning convolutions -- against the oracle.
 
-First green hardware run: round 2 (gpurun_out/r2_pending.json, summarised in profiles/r2_parity.md).  A failure here is
-red like any other test (round 1 reported these groups through an xfail guard; that guard is gone)."""
+A failure here is red like any other test (nothing is xfail-guarded)."""
 import json
 import os
 
