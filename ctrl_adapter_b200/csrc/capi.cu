@@ -112,12 +112,15 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
   cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
   if (d->nsrc < 1 || d->nsrc > 2) return fail(CA_ERR_INVALID, "nsrc must be 1 or 2");
   if (d->ntaps < 1 || d->ntaps > CA_MAX_TAPS) return fail(CA_ERR_INVALID, "ntaps out of range");
-  if (d->box[0] * d->box[1] * d->box[2] * d->box[3] != 128) return fail(CA_ERR_INVALID, "box product must be 128");
+  if (d->box[0] < 1 || d->box[1] < 1 || d->box[2] < 1 || d->box[3] < 1 ||
+      d->box[0] * d->box[1] * d->box[2] * d->box[3] != 128)
+    return fail(CA_ERR_INVALID, "box extents must be positive with product 128");
   if (!d->a[0] || !d->w || !d->out) return fail(CA_ERR_INVALID, "null tensor pointer");
   const bool geglu = d->act == CA_ACT_GEGLU;
   if (geglu && d->n_out * 2 != d->w_rows) return fail(CA_ERR_INVALID, "GEGLU needs w_rows == 2*n_out");
   if (!geglu && d->n_out != d->w_rows) return fail(CA_ERR_INVALID, "n_out must equal w_rows");
   if ((d->n_out & 7) != 0 && !d->out_fp32) return fail(CA_ERR_INVALID, "n_out must be a multiple of 8");
+  if (geglu && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "GEGLU output is bf16");
 
   ca::GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -175,6 +178,17 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
   if (p.blend_src && !p.blend_alpha) return fail(CA_ERR_INVALID, "blend_src without blend_alpha");
   p.out = d->out;
   p.trace = trace_ptr();
+  {
+    // the bf16 epilogue moves 8 columns per 16-byte access when every base and row stride it touches allows it
+    auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    bool vec = a16(p.out) && a16(p.residual) && a16(p.blend_src) && a16(p.rowvec);
+    for (int i = 0; i < 4; ++i) {
+      vec = vec && (p.ostride[i] % 8) == 0;
+      if (p.residual || p.blend_src) vec = vec && (p.rstride[i] % 8) == 0;
+      if (p.rowvec) vec = vec && (p.vstride[i] % 8) == 0;
+    }
+    p.vec_ok = vec ? 1 : 0;
+  }
 
   CUtensorMap ta[2], tw;
   memset(ta, 0, sizeof(ta));

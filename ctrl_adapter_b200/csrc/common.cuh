@@ -204,6 +204,11 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo
   return d;
 }
 
+// barrier `id` (1..15; 0 is __syncthreads) over `count` threads (a multiple of 32)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>

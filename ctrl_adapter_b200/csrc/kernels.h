@@ -27,6 +27,7 @@ struct GemmParams {
   int n_tiles_n;
   int act;
   int out_fp32;
+  int vec_ok;             // bf16 output: out / residual / blend_src / rowvec bases and strides allow 16-byte access
   float out_scale;
   const float* bias;               // [weight rows] fp32
   const __nv_bfloat16* rowvec;     // broadcast add, indexed through vstride
