@@ -121,6 +121,8 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
   if (!geglu && d->n_out != d->w_rows) return fail(CA_ERR_INVALID, "n_out must equal w_rows");
   if ((d->n_out & 7) != 0 && !d->out_fp32) return fail(CA_ERR_INVALID, "n_out must be a multiple of 8");
   if (geglu && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "GEGLU output is bf16");
+  // the fp32 epilogue has no blend term: refuse rather than silently return the unblended result
+  if (d->blend_src && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "AlphaBlender (blend_src) output is bf16");
 
   ca::GemmParams p;
   memset(&p, 0, sizeof(p));

@@ -1,6 +1,12 @@
 """GPU parity checks of every CUDA kernel against a plain PyTorch fp32 reference of the same op on the same
 bf16-quantised inputs.  Used by tests/test_kernels_gpu.py (pytest -m gpu), by __graft_entry__.smoke() and as a
-stand-alone report:  python -m tests.kernel_checks  [--json out.json]
+stand-alone report:  python -m tests.kernel_checks  [--group gemm|conv|attn|misc|layouts]  [--json out.json]
+
+The `layouts` group (LAYOUT_CHECKS, run by tests/test_kernel_layouts_gpu.py) calls the kernels the way the pipelines
+do -- Q/K/V as views of one fused projection, shared per-clip contexts, 17..32 frames, every bf16 GEMM epilogue
+through both store paths -- against float64 references.  The checks run on DEVICE; tests/test_kernel_checks_cpu.py
+sets it to "cpu" and runs them at reduced sizes over tests/ops_emulator.py to show that each one passes a correct
+implementation and fails deliberately wrong ones.
 
 Tolerances (stated per check, torch.testing semantics |out-ref| <= atol + rtol*|ref|):
   * fp32-output contractions: rtol 1e-3 / atol 1e-4 (north-star tolerance; fp32 accumulate on both sides)
@@ -21,7 +27,9 @@ import torch
 import torch.nn.functional as F
 
 BF16 = torch.bfloat16
+F64 = torch.float64
 RESULTS = []
+DEVICE = "cuda"  # where inputs and references live (the CPU tests point this at "cpu" and patch in the emulator)
 
 
 def _ops():
@@ -29,10 +37,15 @@ def _ops():
     return ops
 
 
+def _sync():
+    if torch.device(DEVICE).type == "cuda":
+        torch.cuda.synchronize()
+
+
 def _rand(*shape, scale=1.0, seed=None, dtype=BF16):
-    g = torch.Generator(device="cuda")
+    g = torch.Generator(device=DEVICE)
     g.manual_seed(seed if seed is not None else (hash(shape) & 0xFFFF) + 17)
-    return (torch.randn(*shape, generator=g, device="cuda", dtype=torch.float32) * scale).to(dtype)
+    return (torch.randn(*shape, generator=g, device=DEVICE, dtype=torch.float32) * scale).to(dtype)
 
 
 def _report(name, out, ref, rtol, atol, extra=None, mag=None):
@@ -83,7 +96,7 @@ def check_linear(m, k, n, *, bn=0, bias=True, out_fp32=True, residual=False, act
         mag = torch.maximum(mag, res.float().abs())
     out = ops.linear(x, w, ops.bias_f32(b), act=ops.ACT_SILU if act == "silu" else ops.ACT_NONE, residual=res,
                      out_fp32=out_fp32, bn=bn)
-    torch.cuda.synchronize()
+    _sync()
     rtol, atol = (1e-3, 1e-4) if out_fp32 else (2 ** -6 if residual else 2 ** -7, 1e-3)
     return _report(f"linear m{m} k{k} n{n} bn{bn} {'f32' if out_fp32 else 'bf16'} act={act} res={int(residual)}",
                    out, ref, rtol, atol, mag=mag)
@@ -99,7 +112,7 @@ def check_geglu(m, k, d, seed=0):
     # the same contraction (same kernel, tiles and summation order) with the fp32 pre-activation as output
     pre = ops.linear(x, wi, ops.bias_f32(bi), out_fp32=True, bn=256).reshape(m, d // 128, 2, 128)
     pre = torch.cat([pre[:, :, 0].reshape(m, d), pre[:, :, 1].reshape(m, d)], dim=1)  # undo the per-tile interleave
-    torch.cuda.synchronize()
+    _sync()
     # (1) the contraction against the exact (fp64) pre-activation at the fp32 GEMM tolerance of check_linear
     exact = (x.double() @ w.double().t() + b.double()).float()
     _report(f"geglu pre-activation m{m} k{k} d{2 * d}", pre, exact, 1e-3, 1e-4)
@@ -122,7 +135,7 @@ def check_linear_rowvec(m, k, n, rpv, seed=0):
     lin = (x.float() @ w.float().t()).to(BF16).float()
     ref = (lin + rv.float().repeat_interleave(rpv, dim=0)).to(BF16).float()
     out = ops.linear(x, w, None, rowvec=rv, rows_per_vec=rpv)
-    torch.cuda.synchronize()
+    _sync()
     return _report(f"linear+rowvec m{m} k{k} n{n} rpv{rpv}", out, ref, 2 ** -6, 1e-3, mag=lin)
 
 
@@ -132,12 +145,12 @@ def check_linear_blend(m, k, n, seed=0):
     w = _rand(n, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
     res = _rand(m, n, seed=seed + 4)
     xs = _rand(m, n, seed=seed + 5)
-    alpha = torch.sigmoid(torch.tensor([0.3], device="cuda")).to(BF16)
+    alpha = torch.sigmoid(torch.tensor([0.3], device=DEVICE)).to(BF16)
     lin = (x.float() @ w.float().t()).to(BF16).float()
     xt = (lin + res.float()).to(BF16)
     ref = ((alpha * xs).to(BF16) + ((1.0 - alpha).to(BF16) * xt).to(BF16)).float()
     out = ops.linear(x, w, None, residual=res, blend_src=xs, blend_alpha=alpha.float())
-    torch.cuda.synchronize()
+    _sync()
     mag = torch.maximum(torch.maximum(xt.float().abs(), res.float().abs()), xs.float().abs())
     mag = torch.maximum(mag, lin.abs())  # bf16(x @ w^T) is the first rounded intermediate of the epilogue
     return _report(f"linear+res+blend m{m} k{k} n{n}", out, ref, 2 ** -7, 1e-3, mag=mag)
@@ -178,7 +191,7 @@ def check_conv(n, h, w, cin, cout, *, ksize=3, stride=1, cin2=0, out_fp32=True, 
     wp = ops.pack_conv_weight(wt, kpad)
     out = ops.conv2d(_nhwc(x), wp, ops.bias_f32(b), ksize=ksize, stride=stride, x2=_nhwc(x2) if x2 is not None else None,
                      out_fp32=out_fp32, rowvec=rv, residual=_nhwc(res) if res is not None else None, out_scale=scale)
-    torch.cuda.synchronize()
+    _sync()
     rtol, atol = (1e-3, 1e-4) if out_fp32 else (2 ** -6 if (rowvec or residual) else 2 ** -7, 1e-3)
     return _report(f"conv{ksize}x{ksize} s{stride} n{n} {h}x{w} c{cin}+{cin2}->{cout} {'f32' if out_fp32 else 'bf16'}"
                    f" rv={int(rowvec)} res={int(residual)} sc={scale}", out.permute(0, 3, 1, 2), ref, rtol, atol, mag=mag)
@@ -195,7 +208,7 @@ def check_temporal_conv(b, f, h, w, c, cout, seed=0):
     ref = (ref + rv.float().reshape(b, f, cout).permute(0, 2, 1)[:, :, :, None, None]).to(BF16).float()
     xl = x.permute(0, 2, 3, 4, 1).reshape(b * f, h, w, c).contiguous()
     out = ops.temporal_conv(xl, ops.pack_conv_weight(wt), ops.bias_f32(bias), f, rowvec=rv)
-    torch.cuda.synchronize()
+    _sync()
     out5 = out.reshape(b, f, h, w, cout).permute(0, 4, 1, 2, 3)
     return _report(f"temporal_conv b{b} f{f} {h}x{w} c{c}->{cout}", out5, ref, 2 ** -6, 1e-3, mag=mag)
 
@@ -224,7 +237,7 @@ def check_attention(b, heads, lq, lk, d, seed=0, ramp=0.0):
     def pad(t):
         return F.pad(t, (0, dp - d)).reshape(t.shape[0], t.shape[1], heads * dp).contiguous()
     out = ops.attention(pad(q), pad(k), pad(v), heads, dp, scale)
-    torch.cuda.synchronize()
+    _sync()
     out = out.reshape(b, lq, heads, dp)[..., :d]
     # ramped logits give nearly one-hot rows: the output is a bf16-rounded V row (|v| up to ~4.6, half-ulp 9e-3), so the
     # absolute floor follows torch's own bf16 SDPA error instead of the iid-case 2e-3
@@ -240,10 +253,10 @@ def check_attention(b, heads, lq, lk, d, seed=0, ramp=0.0):
 def check_softmax_rows(rows, cols, seed=0):
     ops = _ops()
     g = torch.Generator(device="cpu").manual_seed(seed + 9)
-    x = (torch.randn(rows, cols, generator=g) * 4.0).cuda()
+    x = (torch.randn(rows, cols, generator=g) * 4.0).to(DEVICE)
     x[0, :7] = 30.0  # a few dominant scores in one row
     out = ops.softmax_rows(x)
-    torch.cuda.synchronize()
+    _sync()
     return _report(f"softmax_rows {rows}x{cols}", out, torch.softmax(x, dim=-1), 2 ** -8, 1e-6)
 
 
@@ -259,7 +272,7 @@ def check_temporal_attention(clips, frames, hw, heads, seed=0):
     p = torch.softmax(to_seq(q) @ to_seq(k).transpose(-1, -2) * 0.125, dim=-1)
     ref = (p @ to_seq(v)).permute(0, 3, 1, 2, 4).reshape(clips * frames, hw, c)
     out = ops.temporal_attention(q.reshape(-1, c), k.reshape(-1, c), v.reshape(-1, c), clips, frames, hw, heads, 0.125)
-    torch.cuda.synchronize()
+    _sync()
     # 16-key softmax with O(1) values: bf16 P rounding alone gives ~4e-3 absolute error
     return _report(f"temporal_attention b{clips} f{frames} hw{hw} h{heads}", out.reshape(ref.shape), ref, 2e-2, 6e-3)
 
@@ -288,7 +301,7 @@ def check_groupnorm(n, h, w, c, *, c2=0, silu=True, up=False, imgs_per_sample=1,
     ref = ref.to(BF16).float()
     out = ops.group_norm(_nhwc(x), gamma, beta, eps, silu=silu, up2x=up, x2=_nhwc(x2) if x2 is not None else None,
                          imgs_per_sample=imgs_per_sample)
-    torch.cuda.synchronize()
+    _sync()
     return _report(f"groupnorm n{n} {h}x{w} c{c}+{c2} silu={int(silu)} up={int(up)} ips={imgs_per_sample}",
                    out.permute(0, 3, 1, 2), ref, 2 ** -7, 2e-3)
 
@@ -308,7 +321,7 @@ def check_layernorm(rows, c, *, add=False, seed=0):
     else:
         out = ops.layer_norm(x, gamma, beta, 1e-5)
     ref = F.layer_norm(xin, (c,), gamma, beta, 1e-5).to(BF16).float()
-    torch.cuda.synchronize()
+    _sync()
     return _report(f"layernorm rows{rows} c{c} add={int(add)}", out, ref, 2 ** -7, 2e-3)
 
 
@@ -319,24 +332,24 @@ def check_frame_conv_small(clips, frames, h, w, cin=3, cout=3, seed=0):
     b = (_rand(cout, seed=seed + 3, dtype=torch.float32) * 0.3).to(BF16).float().cpu().contiguous()
     y = ops.frame_conv_small(x, wt, b, frames, cin)
     xs = x[..., :cin].float().reshape(clips, frames, h, w, cin).permute(0, 4, 1, 2, 3)
-    ref = F.conv3d(xs, wt.cuda()[:, :, :, None, None], b.cuda(), padding=(1, 0, 0))
+    ref = F.conv3d(xs, wt.to(DEVICE)[:, :, :, None, None], b.to(DEVICE), padding=(1, 0, 0))
     ref = ref.permute(0, 2, 1, 3, 4).reshape(clips * frames, cout, h, w).to(BF16).float()
-    torch.cuda.synchronize()
+    _sync()
     return _report(f"frame_conv_small {clips}x{frames} frames {h}x{w} {cin}->{cout}", y, ref, 2 ** -7, 2e-3)
 
 
 def check_timestep_embedding(seed=0):
     ops = _ops()
-    t = torch.tensor([999.0, 981.0, 501.0, 1.0, 0.0, 13.0], device="cuda")
+    t = torch.tensor([999.0, 981.0, 501.0, 1.0, 0.0, 13.0], device=DEVICE)
     recs = []
     for dim, round_t in ((320, False), (320, True), (1280, True), (256, False)):
         tt = t.to(BF16).float() if round_t else t
         half = dim // 2
-        freq = torch.exp(-math.log(10000.0) * torch.arange(half, device="cuda", dtype=torch.float32) / half)
+        freq = torch.exp(-math.log(10000.0) * torch.arange(half, device=DEVICE, dtype=torch.float32) / half)
         arg = tt[:, None] * freq[None, :]
         ref = torch.cat([torch.cos(arg), torch.sin(arg)], dim=-1).to(BF16).float()
         out = ops.timestep_embedding(t, dim, flip_sin_to_cos=True, freq_shift=0.0, round_t_bf16=round_t)
-        torch.cuda.synchronize()
+        _sync()
         recs.append(_report(f"timestep_embedding dim{dim} round_t={int(round_t)}", out, ref, 2 ** -7, 4e-3))
     return recs[-1]
 
@@ -359,26 +372,26 @@ def check_layout_pool(seed=0):
     a, b = _rand(1000, 64, seed=5), _rand(1000, 64, seed=6)
     _report("add", ops.add(a, b), (a.float() + b.float()).to(BF16), 0.0, 0.0)
     _report("silu", ops.silu(a), F.silu(a.float()).to(BF16), 2 ** -7, 1e-3)
-    torch.cuda.synchronize()
+    _sync()
 
 
 def check_router(seed=0):
     ops = _ops()
     logits = _rand(13, 7, seed=seed + 1, dtype=torch.float32)
-    mask = torch.tensor([1, 1, 0, 1, 0, 0, 0], dtype=torch.uint8, device="cuda")
+    mask = torch.tensor([1, 1, 0, 1, 0, 0, 0], dtype=torch.uint8, device=DEVICE)
     masked = logits.clone()
     masked[:, mask == 0] -= 1e6
     ref = torch.softmax(masked, dim=-1)
     out = ops.router_weights(logits, mask)
     _report("router_weights", out, ref, 1e-5, 1e-7)
     xs = [_rand(4, 8, 8, 64, seed=seed + 10 + i) for i in range(3)]
-    w = torch.tensor([0.5, 0.3, 0.2], device="cuda")
+    w = torch.tensor([0.5, 0.3, 0.2], device=DEVICE)
     acc = None
     for x, wk in zip(xs, w.to(BF16)):
         term = (x * wk)
         acc = term if acc is None else acc + term
     out = ops.router_merge(xs, w)
-    torch.cuda.synchronize()
+    _sync()
     _report("router_merge", out, acc, 0.0, 0.0)
 
 
@@ -388,23 +401,440 @@ def check_cfg(seed=0):
     lat = _rand(2, 4, 16, 16, seed=seed + 3, dtype=torch.float32).to(BF16).float()
     g, sigma, sigma_next = 5.0, 3.2, 2.7
     div = math.sqrt(sigma_next ** 2 + 1)
-    row = torch.tensor([981.0, sigma, sigma_next, div], device="cuda")
+    row = torch.tensor([981.0, sigma, sigma_next, div], device=DEVICE)
     eps = (eu + (g * (et - eu)).to(BF16)).to(BF16)
-    x0 = lat - (torch.tensor(sigma, device="cuda") * eps).float()  # 0-dim fp32 * bf16 tensor -> bf16
+    x0 = lat - (torch.tensor(sigma, device=DEVICE) * eps).float()  # 0-dim fp32 * bf16 tensor -> bf16
     ref = (lat + (lat - x0) / sigma * (sigma_next - sigma)).to(BF16)
     nxt = torch.empty_like(eu)
     out = ops.cfg_euler(eu, et, lat, g, row, model_in_next=nxt)
-    torch.cuda.synchronize()
+    _sync()
     _report("cfg_euler (bf16 latents)", out, ref, 2 ** -7, 1e-3)
-    _report("cfg_euler next_in", nxt, (ref / torch.tensor(div, device="cuda")).to(BF16), 2 ** -7, 1e-3)
+    _report("cfg_euler next_in", nxt, (ref / torch.tensor(div, device=DEVICE)).to(BF16), 2 ** -7, 1e-3)
     a_t, a_prev = 0.3, 0.45
-    row = torch.tensor([500.0, a_t, a_prev, 1.0], device="cuda")
+    row = torch.tensor([500.0, a_t, a_prev, 1.0], device=DEVICE)
     epsf = eps.float()
     x0 = (lat - math.sqrt(1 - a_t) * epsf) / math.sqrt(a_t)
     ref = math.sqrt(a_prev) * x0 + math.sqrt(1 - a_prev) * epsf
     out = ops.cfg_ddim(eu, et, lat, g, row, round_latents_bf16=False)
-    torch.cuda.synchronize()
+    _sync()
     _report("cfg_ddim (fp32 latents)", out, ref, 1e-5, 1e-5)
+
+
+# ------------------------------------------------------------------------------------------------
+# layouts and variants the pipelines call the kernels with: float64 references on the same bf16 inputs, bf16 rounding
+# applied at the kernels' rounding points (the ones tests/ops_emulator.py lists per op), tolerances of the header
+# ------------------------------------------------------------------------------------------------
+def _r64(t):
+    """round to bf16, keep computing in float64"""
+    return t.to(BF16).to(F64)
+
+
+def _exact(name, ok, extra=None):
+    rec = {"check": name, "ok": bool(ok)}
+    if extra:
+        rec.update(extra)
+    RESULTS.append(rec)
+    return rec
+
+
+def _default_bn(w_rows, geglu=False):
+    """the tile width ca_gemm picks when bn = 0"""
+    if geglu or w_rows % 256 == 0:
+        return 256
+    if w_rows % 160 == 0:
+        return 160
+    if w_rows % 128 == 0:
+        return 128
+    return 64 if w_rows <= 64 else 128 if w_rows <= 128 else 256
+
+
+def _attn_ref64(q, k, v, kv_idx, scale, chunk=256):
+    """q [B, Lq, H, d], k / v [Bk, Lk, H, d]; query batch b attends to K/V batch kv_idx[b].  float64, query axis in chunks
+    so that the score matrix stays small."""
+    qd = q.to(F64).permute(0, 2, 1, 3)
+    kd = k.to(F64).permute(0, 2, 1, 3)[kv_idx]
+    vd = v.to(F64).permute(0, 2, 1, 3)[kv_idx]
+    out = torch.empty(qd.shape[:3] + (vd.shape[3],), dtype=F64, device=q.device)
+    for i in range(0, qd.shape[2], chunk):
+        p = torch.softmax(qd[:, :, i:i + chunk] @ kd.transpose(-1, -2) * scale, dim=-1)
+        out[:, :, i:i + chunk] = p @ vd
+    return out.permute(0, 2, 1, 3)
+
+
+def _attn_verdict(name, q, k, v, kv_idx, scale, out):
+    """check_attention's criteria (rtol 2e-2 / atol 2e-3, and at most 2x the error of torch's bf16 SDPA on the same
+    inputs), the SDPA bound applied to every (batch, head) on its own so that one wrong head cannot hide in the totals."""
+    ref = _attn_ref64(q, k, v, kv_idx, scale)
+    sd = F.scaled_dot_product_attention(*(t.permute(0, 2, 1, 3) for t in (q, k[kv_idx], v[kv_idx])), scale=scale)
+    err_bh = (out.to(F64) - ref).abs().amax(dim=(1, 3))              # [B, H]
+    sd_bh = (sd.permute(0, 2, 1, 3).to(F64) - ref).abs().amax(dim=(1, 3))
+    ratio = err_bh / (2.0 * sd_bh + 1e-3)
+    wb, wh = divmod(int(err_bh.argmax()), err_bh.shape[1])
+    rb, rh = divmod(int(ratio.argmax()), ratio.shape[1])
+    rec = _report(name, out, ref, 2e-2, 2e-3, {
+        "sdpa_bf16_max_err": float(sd_bh.max()), "worst_bh": f"b{wb}h{wh}", "worst_bh_err": float(err_bh[wb, wh]),
+        "worst_bh_sdpa_err": float(sd_bh[wb, wh]), "max_bh_err_over_2x_sdpa": float(ratio[rb, rh]),
+        "max_ratio_bh": f"b{rb}h{rh}"})
+    if float(ratio.max()) > 1.0:
+        rec["ok"] = False
+        rec["why"] = f"(batch, head) b{rb}h{rh}: error larger than 2x torch bf16 SDPA"
+    return rec
+
+
+def _pad_heads(t, dp):
+    """[B, L, H, d] -> [B, L, H, dp]: the zero-padded head layout the packed projection weights produce"""
+    return F.pad(t, (0, dp - t.shape[-1]))
+
+
+def check_attention_fused_qkv(b, heads, l, d, seed=0):
+    """Self-attention on Q / K / V column views of ONE [B, L, 3 * H * Dp] projection (row stride 3 * H * Dp), as
+    layers.Attention.forward slices them."""
+    ops = _ops()
+    dp = (d + 63) // 64 * 64
+    inner = heads * dp
+    q, k, v = (_rand(b, l, heads, d, seed=seed + i) for i in (1, 2, 3))
+    qkv = torch.stack([_pad_heads(t, dp) for t in (q, k, v)], dim=2).reshape(b, l, 3 * inner)
+    out = ops.attention(qkv[:, :, :inner], qkv[:, :, inner:2 * inner], qkv[:, :, 2 * inner:], heads, dp, d ** -0.5)
+    _sync()
+    out = out.reshape(b, l, heads, dp)[..., :d]
+    return _attn_verdict(f"attention fused-qkv b{b} h{heads} l{l} d{d}", q, k, v, torch.arange(b, device=q.device),
+                         d ** -0.5, out)
+
+
+def check_attention_cross_kv(b, heads, lq, lk, d, kv_batch_div=1, seed=0):
+    """Cross-attention with K / V as the two halves of one [B / kv_batch_div, Lk, 2 * H * Dp] projection of the context.
+    kv_batch_div > 1: the frames of a clip share their clip's context, and every clip's context is different."""
+    ops = _ops()
+    dp = (d + 63) // 64 * 64
+    inner = heads * dp
+    bk = b // kv_batch_div
+    q = _rand(b, lq, heads, d, seed=seed + 1)
+    k, v = _rand(bk, lk, heads, d, seed=seed + 2), _rand(bk, lk, heads, d, seed=seed + 3)
+    kv = torch.stack([_pad_heads(t, dp) for t in (k, v)], dim=2).reshape(bk, lk, 2 * inner)
+    out = ops.attention(_pad_heads(q, dp).reshape(b, lq, inner), kv[:, :, :inner], kv[:, :, inner:], heads, dp,
+                        d ** -0.5, kv_batch_div=kv_batch_div)
+    _sync()
+    out = out.reshape(b, lq, heads, dp)[..., :d]
+    kv_idx = torch.arange(b, device=q.device) // kv_batch_div
+    return _attn_verdict(f"attention cross-kv b{b} h{heads} lq{lq} lk{lk} d{d} kv_div{kv_batch_div}", q, k, v, kv_idx,
+                         d ** -0.5, out)
+
+
+def check_temporal_attention_fused(clips, frames, hw, heads, seed=0):
+    """Frame-axis attention on Q / K / V column views of one [rows, 3 * inner] projection (row_stride 3 * inner), as the
+    temporal transformers of the UNets and the video adapter call it.  Tolerance of check_temporal_attention."""
+    ops = _ops()
+    inner = heads * 64
+    qkv = _rand(clips * frames * hw, 3 * inner, seed=seed + 1)
+    q, k, v = qkv[:, :inner], qkv[:, inner:2 * inner], qkv[:, 2 * inner:]
+    out = ops.temporal_attention(q, k, v, clips, frames, hw, heads, 0.125, row_stride=3 * inner)
+    _sync()
+
+    def seq(t):  # rows (clip, frame, pixel) -> [clip, pixel, head, frame, 64]
+        return t.to(F64).reshape(clips, frames, hw, heads, 64).permute(0, 2, 3, 1, 4)
+    p = torch.softmax(seq(q) @ seq(k).transpose(-1, -2) * 0.125, dim=-1)
+    ref = (p @ seq(v)).permute(0, 3, 1, 2, 4).reshape(clips * frames * hw, inner)
+    err_f = (out.to(F64) - ref).abs().reshape(clips, frames, -1).amax(dim=(0, 2))  # worst error per frame
+    wf = int(err_f.argmax())
+    return _report(f"temporal_attention fused-qkv b{clips} f{frames} hw{hw} h{heads}", out, ref, 2e-2, 6e-3,
+                   {"worst_frame": wf, "worst_frame_err": float(err_f[wf])})
+
+
+EPILOGUES = ("bias", "bias_silu", "bias_scale", "bias_scale_res", "rowvec", "bias_res", "rowvec_res", "bias_res_blend",
+             "rowvec_res_blend", "geglu")
+
+
+def check_gemm_epilogue(kind, m, k, n, rows_per_vec=0, seed=0):
+    """One bf16 GEMM epilogue combination (`kind`: parts of EPILOGUES joined by '_'), run twice.  The first run writes a
+    fresh aligned output and is checked against the float64 reference.  The second writes channels [4, 4 + n) of a
+    wider buffer, with the residual / blend source / row vector at the same offset in buffers of that width: the 8-byte
+    base offset sends the storers down the element-wise drain, which must reproduce the first run bit for bit and leave
+    the bytes around the slice alone."""
+    ops = _ops()
+    parts = kind.split("_")
+    geglu = kind == "geglu"
+    x = _rand(m, k, seed=seed + 1)
+    w_rows = 2 * n if geglu else n
+    w = _rand(w_rows, k, scale=k ** -0.5, seed=seed + 2)
+    b = _rand(w_rows, seed=seed + 3) if ("bias" in parts or geglu) else None
+    scale = 0.7 if "scale" in parts else 1.0
+    rv = _rand(m // rows_per_vec, n, seed=seed + 4) if "rowvec" in parts else None
+    res = _rand(m, n, seed=seed + 5) if "res" in parts else None
+    xs = _rand(m, n, seed=seed + 6) if "blend" in parts else None
+    alpha = torch.sigmoid(torch.tensor([0.3], device=DEVICE)).to(BF16).float() if xs is not None else None
+    act = ops.ACT_GEGLU if geglu else ops.ACT_SILU if "silu" in parts else ops.ACT_NONE
+    wk, bk = ops.pack_geglu_weight(w, b, 256) if geglu else (w, b)
+    bias = ops.bias_f32(bk)
+    kw = dict(act=act, out_scale=scale, rows_per_vec=rows_per_vec, blend_alpha=alpha)
+    out = ops.linear(x, wk, bias, rowvec=rv, residual=res, blend_src=xs, **kw)
+
+    def slot(t):  # the same values in columns [4, 4 + n) of an [rows, n + 16] buffer
+        if t is None:
+            return None
+        buf = _rand(t.shape[0], n + 16, seed=seed + 9)
+        buf[:, 4:4 + n] = t
+        return buf[:, 4:4 + n]
+    obuf = torch.full((m, n + 16), 7.0, device=DEVICE, dtype=BF16)
+    ops.linear(x, wk, bias, rowvec=slot(rv), residual=slot(res), blend_src=slot(xs), out=obuf[:, 4:4 + n], **kw)
+    _sync()
+    name = f"gemm epilogue {kind} m{m} k{k} n{n} bn{_default_bn(w_rows, geglu)}"
+
+    if geglu:
+        # as check_geglu: the contraction against fp64 (fp32 output of the same kernel and tiles), then the epilogue's
+        # rounding chain applied to the pre-activation the kernel accumulated
+        pre = ops.linear(x, wk, bias, out_fp32=True).reshape(m, n // 128, 2, 128)
+        pre = torch.cat([pre[:, :, 0].reshape(m, n), pre[:, :, 1].reshape(m, n)], dim=1)
+        _sync()
+        exact = x.to(F64) @ w.to(F64).t() + b.to(BF16).to(F64)
+        _report(f"{name} pre-activation", pre, exact, 1e-3, 1e-4)
+        h = _r64(pre.to(F64))
+        ref = _r64(h[:, :n] * _r64(F.gelu(h[:, n:])))
+        _report(name, out, ref, 2 ** -6, 2e-3)
+    else:
+        v = x.to(F64) @ w.to(F64).t()
+        if bias is not None:
+            v = v + bias.to(F64)
+        if "silu" in parts or scale != 1.0:
+            # as for GEGLU: SiLU or the scale round a second time, and carry a 1-ulp flip of a pre-activation within an
+            # fp32 ulp of a bf16 tie (which way it rounds depends on the summation order) past the output tolerance.
+            # So the contraction is checked on its own, and the chain is applied to the pre-activation the kernel
+            # accumulated (fp32 output of the same kernel: same tiles, same summation order).
+            pre = ops.linear(x, wk, bias, out_fp32=True)
+            _sync()
+            _report(f"{name} pre-activation", pre, v, 1e-3, 1e-4)
+            v = pre.to(F64)
+        v = _r64(v)
+        if "silu" in parts:
+            v = _r64(F.silu(v))
+        if scale != 1.0:
+            v = _r64(v * scale)
+        mag = v.abs()
+        if rv is not None:
+            v = _r64(v + rv.to(F64).repeat_interleave(rows_per_vec, dim=0))
+            mag = torch.maximum(mag, v.abs())
+        if res is not None:
+            v = _r64(v + res.to(F64))
+            mag = torch.maximum(torch.maximum(mag, res.to(F64).abs()), v.abs())
+        if xs is not None:
+            a = alpha.to(F64)
+            v = _r64(_r64(a * xs.to(F64)) + _r64(_r64(1.0 - a) * v))
+            mag = torch.maximum(torch.maximum(mag, xs.to(F64).abs()), v.abs())
+        # one rounding: 1 ulp; bias + rounding + blend: check_linear_blend's 1 ulp of the largest intermediate; a row
+        # vector and / or residual before it: 2 ulps of the largest intermediate (check_conv / check_linear_rowvec)
+        multi = rv is not None or (res is not None and xs is None)
+        _report(name, out, v, 2 ** -6 if multi else 2 ** -7, 1e-3, mag=mag if (multi or xs is not None) else None)
+    same = torch.equal(obuf[:, 4:4 + n].view(torch.int16), out.view(torch.int16))
+    n_diff = int((obuf[:, 4:4 + n].view(torch.int16) != out.view(torch.int16)).sum())
+    untouched = bool((obuf[:, :4] == 7.0).all()) and bool((obuf[:, 4 + n:] == 7.0).all())
+    return _exact(f"{name} element-wise drain == aligned, bytes around the slice kept", same and untouched,
+                  {"n_diff": n_diff, "n": out.numel(), "untouched": untouched})
+
+
+def check_temporal_conv_epilogue(b, f, h, w, c, cout, seed=0):
+    """Conv3d (3,1,1) over the frames with row vector + residual + AlphaBlender in one epilogue (the temporal ResNet's
+    convs in the video adapter).  f = 1: both frame taps fall on the zero padding."""
+    ops = _ops()
+    x = _rand(b * f, h, w, c, seed=seed + 1)
+    wt = _rand(cout, c, 3, 1, 1, scale=(3 * c) ** -0.5, seed=seed + 2)
+    bias = ops.bias_f32(_rand(cout, seed=seed + 3))
+    rv = _rand(b * f, cout, seed=seed + 4)
+    res = _rand(b * f, h, w, cout, seed=seed + 5)
+    xs = _rand(b * f, h, w, cout, seed=seed + 6)
+    alpha = torch.sigmoid(torch.tensor([-0.4], device=DEVICE)).to(BF16).float()
+    out = ops.temporal_conv(x, ops.pack_conv_weight(wt), bias, f, rowvec=rv, residual=res, blend_src=xs,
+                            blend_alpha=alpha)
+    _sync()
+    xp = F.pad(x.to(F64).reshape(b, f, h * w, c), (0, 0, 0, 0, 1, 1))  # a zero frame at both ends of every clip
+    wd = wt.to(F64)[:, :, :, 0, 0]
+    acc = sum(xp[:, t:t + f] @ wd[:, :, t].t() for t in range(3)) + bias.to(F64)
+    v = _r64(acc)
+    mag = v.abs()
+    v = _r64(v + rv.to(F64).reshape(b, f, 1, cout))
+    mag = torch.maximum(mag, v.abs())
+    resd, xsd = res.to(F64).reshape(b, f, h * w, cout), xs.to(F64).reshape(b, f, h * w, cout)
+    v = _r64(v + resd)
+    mag = torch.maximum(torch.maximum(mag, v.abs()), resd.abs())
+    a = alpha.to(F64)
+    v = _r64(_r64(a * xsd) + _r64(_r64(1.0 - a) * v))
+    mag = torch.maximum(torch.maximum(mag, v.abs()), xsd.abs())
+    return _report(f"temporal_conv rowvec+res+blend b{b} f{f} {h}x{w} c{c}->{cout}", out.reshape(v.shape), v,
+                   2 ** -6, 1e-3, mag=mag)
+
+
+def check_linear_f32_scale(m, n, k, seed=0):
+    """fp32 output with out_scale: the attention scores q k^T * C^-0.5 of the VAE mid block."""
+    ops = _ops()
+    q, kk = _rand(m, k, seed=seed + 1), _rand(n, k, seed=seed + 2)
+    out = ops.linear(q, kk, None, out_fp32=True, out_scale=k ** -0.5)
+    _sync()
+    ref = (q.to(F64) @ kk.to(F64).t()) * k ** -0.5
+    return _report(f"linear f32 out_scale m{m} n{n} k{k}", out, ref, 1e-3, 1e-4)
+
+
+def _bf16_ulp(a):
+    e = torch.frexp(a.abs().clamp_min(2.0 ** -126))[1]
+    return torch.ldexp(torch.ones_like(a), e - 8)
+
+
+def check_cfg_ddim_layout(v_prediction, bf16_latents, shape=(2, 4, 16, 32, 32), seed=0):
+    """Classifier-free guidance + DDIM step as the I2VGen-XL loop runs it.  bf16 latents: within 1 bf16 ulp of the
+    float64 chain with the kernel's rounding points (ulp of the largest intermediate of the chain, so that a quotient
+    rounded to one side of a tie in fp32 cannot fail it); fp32 latents: rtol 1e-6 of the chain's term magnitudes."""
+    ops = _ops()
+    eu, et = _rand(*shape, seed=seed + 1), _rand(*shape, seed=seed + 2)
+    lat = _rand(*shape, seed=seed + 3, dtype=torch.float32)
+    if bf16_latents:
+        lat = lat.to(BF16).float()
+    g, a_t, a_prev = 9.0, 0.3, 0.45
+    row = torch.tensor([500.0, a_t, a_prev, 0.0], device=DEVICE)
+    nxt = torch.empty(shape, device=DEVICE, dtype=BF16)
+    out = ops.cfg_ddim(eu, et, lat, g, row, model_in_next=nxt, round_latents_bf16=bf16_latents,
+                       v_prediction=v_prediction)
+    _sync()
+    rr = _r64 if bf16_latents else (lambda t: t)
+    at32, ap32 = row[1:2].cpu(), row[2:3].cpu()  # the fp32 values the kernel reads; 1 - a is an fp32 subtraction
+    sa, sb, sap, sbp = (rr(t.to(F64).sqrt().to(DEVICE)) for t in (at32, 1.0 - at32, ap32, 1.0 - ap32))
+    u, c, x = eu.to(F64), et.to(F64), lat.to(F64)
+    mo = _r64(u + _r64(g * _r64(c - u)))
+    if v_prediction:
+        x0 = rr(rr(sa * x) - rr(sb * mo))
+        eps = rr(rr(sa * mo) + rr(sb * x))
+        terms = [sap * (sa * x.abs() + sb * mo.abs()), sbp * (sa * mo.abs() + sb * x.abs())]
+    else:
+        x0 = rr(rr(x - rr(sb * mo)) / sa)
+        eps = mo
+        terms = [sap * (x.abs() + sb * mo.abs()) / sa, sbp * mo.abs()]
+    t1, t2 = rr(sap * x0), rr(sbp * eps)
+    ref = rr(t1 + t2)
+    name = f"cfg_ddim {'v' if v_prediction else 'epsilon'} {'bf16' if bf16_latents else 'fp32'} latents"
+    err = (out.to(F64) - ref).abs()
+    if bf16_latents:
+        big = torch.stack([ref.abs(), x0.abs(), eps.abs(), t1.abs(), t2.abs()]).amax(dim=0)
+        tol = _bf16_ulp(big)
+    else:
+        tol = 1e-6 * torch.maximum(ref.abs(), terms[0] + terms[1])
+    bad = int((err > tol).sum()) + int((~torch.isfinite(out)).sum())
+    nxt_ok = torch.equal(nxt, out.to(BF16))
+    return _exact(name, bad == 0 and nxt_ok, {"max_abs_err": float(err.max()), "max_err_over_tol": float((err / tol).max()),
+                                             "n_bad": bad, "n": out.numel(), "model_in_next_exact": nxt_ok})
+
+
+def _latent_encoder_ref64(x, clips, frames, params):
+    """float64 restatement of the I2VGen-XL image-latent encoder with the kernel's bf16 rounding points (ops_emulator
+    lists them).  Returns y [clips, pixel, frame, 4] and, per output row, the largest magnitude of its intermediates."""
+    n, h, w_, _ = x.shape
+    p = params.to(F64)
+    sizes = [("ln_w", 4), ("ln_b", 4), ("wq", 32), ("wk", 32), ("wv", 32), ("wo", 32), ("bo", 4), ("w1", 64), ("b1", 16),
+             ("w2", 64), ("b2", 4)]
+    o, prm = 0, {}
+    for key, sz in sizes:
+        prm[key] = p[o:o + sz]
+        o += sz
+    wq, wk, wv = (prm[key].reshape(8, 4) for key in ("wq", "wk", "wv"))
+    wo, w1, w2 = prm["wo"].reshape(4, 8), prm["w1"].reshape(16, 4), prm["w2"].reshape(4, 16)
+    xs = x[..., :4].to(F64).reshape(clips, frames, h * w_, 4).permute(0, 2, 1, 3)  # [clip, pixel, frame, 4]
+    xn = _r64(F.layer_norm(xs, (4,), prm["ln_w"], prm["ln_b"], 1e-5))
+    q, k, v = (_r64(xn @ m.t()) for m in (wq, wk, wv))
+
+    def heads(t):
+        return t.reshape(*t.shape[:-1], 2, 4).transpose(-2, -3)  # [clip, pixel, head, frame, 4]
+    a = _r64(torch.softmax(heads(q) @ heads(k).transpose(-1, -2) * 0.5, dim=-1) @ heads(v))
+    a = a.transpose(-2, -3).reshape(q.shape)
+    hcur = _r64(_r64(a @ wo.t() + prm["bo"]) + xs)
+    u = _r64(_r64(F.gelu(_r64(hcur @ w1.t() + prm["b1"]))))
+    ff = _r64(u @ w2.t() + prm["b2"])
+    y = _r64(ff + hcur)
+    mag = torch.cat([t.abs() for t in (xs, xn, q, k, v, a, hcur, u, ff, y)], dim=-1).amax(dim=-1, keepdim=True)
+    return y, mag
+
+
+def check_latent_encoder(clips, frames, h=10, w=10, c_stride=8, seed=0):
+    """The I2VGen-XL image-latent encoder (one thread per (clip, pixel); hw = 100 is not a multiple of the 64-thread
+    block).  Channels 4..7 of the input are nonzero; those of the output must be exactly zero."""
+    ops = _ops()
+    x = _rand(clips * frames, h, w, c_stride, seed=seed + 1)
+    scales = [1.0, 1.0, 0.5, 0.5, 0.5, 0.35, 1.0, 0.5, 1.0, 0.25, 1.0]
+    counts = [4, 4, 32, 32, 32, 32, 4, 64, 16, 64, 4]
+    params = torch.cat([_rand(cnt, seed=seed + 10 + i, dtype=torch.float32) * s
+                        for i, (cnt, s) in enumerate(zip(counts, scales))])
+    params[:4] += 1.0  # LayerNorm weight around 1
+    params = params.to(BF16).float().contiguous()
+    out = ops.i2vgen_latent_encoder(x, clips, frames, params)
+    _sync()
+    y, mag = _latent_encoder_ref64(x, clips, frames, params)
+    o4 = out[..., :4].reshape(clips, frames, h * w, 4).permute(0, 2, 1, 3)
+    name = f"i2vgen_latent_encoder b{clips} f{frames} hw{h * w} c_stride{c_stride}"
+    _exact(f"{name} channels 4..{c_stride - 1} zero", bool((out[..., 4:] == 0).all()))
+    return _report(name, o4, y, 2 ** -6, 1e-3, mag=mag.expand_as(y))
+
+
+def check_groupnorm_offset(n, h, w, c, seed=0):
+    """GroupNorm statistics are one-pass fp32 sums of x and x^2 with no shift: half of the groups sit at mean 40 with
+    std 0.5, where E[x^2] - E[x]^2 cancels (mean / std)^2 = 6400-fold.  Tolerance of check_groupnorm."""
+    ops = _ops()
+    grp = torch.arange(c, device=DEVICE) // (c // 32)
+    off = (grp % 2 == 0)
+    mean = torch.where(off, 40.0, 0.0)[None, :, None, None]
+    std = torch.where(off, 0.5, 1.0)[None, :, None, None]
+    x = (_rand(n, c, h, w, seed=seed + 1, dtype=torch.float32) * std + mean).to(BF16)
+    gamma = _rand(c, seed=seed + 2, dtype=torch.float32) * 0.2 + 1.0
+    beta = _rand(c, seed=seed + 3, dtype=torch.float32) * 0.2
+    out = ops.group_norm(_nhwc(x), gamma, beta, 1e-6)
+    _sync()
+    ref = F.group_norm(x.to(F64), 32, gamma.to(F64), beta.to(F64), 1e-6).to(BF16)
+    return _report(f"groupnorm mean40/std0.5 groups n{n} {h}x{w} c{c}", out.permute(0, 3, 1, 2), ref, 2 ** -7, 2e-3)
+
+
+def layout_cases(small=False):
+    """[(name, check)] of the layout checks; small=True: reduced sizes for the CPU run over the emulator (same layouts,
+    same edges: partial tiles, padded head dims, frame counts either side of 16, shared contexts)."""
+    s = small
+    cases = [
+        ("attn_fused_qkv_d64", lambda: check_attention_fused_qkv(2, 3 if s else 10, 200 if s else 1000, 64)),
+        ("attn_fused_qkv_d40", lambda: check_attention_fused_qkv(2, 2 if s else 10, 150 if s else 300, 40)),
+        ("attn_fused_qkv_d160", lambda: check_attention_fused_qkv(2, 2 if s else 10, 150 if s else 300, 160)),
+        ("attn_cross_kv", lambda: check_attention_cross_kv(2, 2 if s else 10, 130 if s else 1000, 77, 64)),
+        ("attn_cross_kv_batch_div", lambda: check_attention_cross_kv(8 if s else 32, 2 if s else 5, 64 if s else 256, 77,
+                                                                     64, kv_batch_div=4 if s else 16)),
+    ]
+    hw = 11 if s else 99  # not a multiple of the pixels per tile (8 for F <= 16, 4 above)
+    for f in (1, 2, 3, 16, 17, 25, 32):
+        cases.append((f"tattn_fused_f{f}", lambda f=f: check_temporal_attention_fused(2, f, hw, 2 if s else 5)))
+    cases.append(("tattn_fused_svd_xt", lambda: check_temporal_attention_fused(1 if s else 2, 25, 36 if s else 576,
+                                                                               2 if s else 5)))
+    gemm = [  # (kind, m, k, n, rows_per_vec): n_out picks BN 160 / 256 / 64 / 128 / 128 / 160 / 256 / 128 / 64 / 256
+        ("bias", 1000, 320, 320, 0), ("bias_silu", 1000, 320, 1280, 0), ("bias_scale", 1000, 256, 64, 0),
+        ("bias_scale_res", 1000, 320, 384, 0), ("rowvec", 1024, 320, 384, 256), ("bias_res", 9000, 640, 640, 0),
+        ("rowvec_res", 8192, 320, 1280, 64), ("bias_res_blend", 1000, 320, 128, 0),
+        ("rowvec_res_blend", 1024, 320, 64, 256), ("geglu", 1000, 320, 1280, 0)]
+    for kind, m, k, n, rpv in gemm:
+        if s:
+            m, k = (256 if rpv else 200), 64
+            rpv = 64 if rpv else 0
+        cases.append((f"gemm_{kind}", lambda a=(kind, m, k, n, rpv): check_gemm_epilogue(*a[:4], rows_per_vec=a[4])))
+    cases += [
+        ("temporal_conv_epilogue_f16", lambda: check_temporal_conv_epilogue(2, 4 if s else 16, 4 if s else 8,
+                                                                            4 if s else 8, 64 if s else 320,
+                                                                            64 if s else 320)),
+        ("temporal_conv_epilogue_f1", lambda: check_temporal_conv_epilogue(2, 1, 4 if s else 8, 4 if s else 8,
+                                                                           64 if s else 320, 64 if s else 320)),
+        ("linear_f32_out_scale", lambda: check_linear_f32_scale(256 if s else 4096, 256 if s else 4096, 512)),
+    ]
+    for vpred in (False, True):
+        for bf in (True, False):
+            cases.append((f"cfg_ddim_{'v' if vpred else 'eps'}_{'bf16' if bf else 'fp32'}",
+                          lambda v=vpred, b=bf: check_cfg_ddim_layout(v, b, (2, 4, 4, 8, 8) if s else (2, 4, 16, 32, 32))))
+    for f in (1, 16, 32):
+        cases.append((f"latent_encoder_f{f}", lambda f=f: check_latent_encoder(2, f)))
+    cases += [
+        ("groupnorm_offset", lambda: check_groupnorm_offset(1 if s else 2, 16 if s else 64, 16 if s else 64,
+                                                            64 if s else 320)),
+        ("groupnorm_offset_vae_plane", lambda: check_groupnorm_offset(1, 32 if s else 512, 32 if s else 512, 128)),
+    ]
+    return cases
+
+
+LAYOUT_CHECKS = layout_cases()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -425,7 +855,7 @@ def run_all(stop_on_fail=False, group=None):
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
     RESULTS.clear()
-    plan = [
+    groups = {"gemm": [
         lambda: check_linear(256, 64, 64),
         lambda: check_linear(128, 128, 128, bias=False),
         lambda: check_linear(1000, 512, 320),
@@ -445,6 +875,7 @@ def run_all(stop_on_fail=False, group=None):
         lambda: check_linear(700, 256, 328, out_fp32=False, residual=True),         # n_out not a multiple of 64
         lambda: check_linear(520, 192, 40, out_fp32=False, bias=False),             # BN 64, single partial unit
         lambda: check_geglu(5000, 640, 2560),
+    ], "conv": [
         lambda: check_conv(2, 16, 16, 64, 64),
         lambda: check_conv(2, 32, 32, 320, 320),
         lambda: check_conv(3, 8, 8, 1280, 1280, out_fp32=False, rowvec=True, residual=True),
@@ -459,6 +890,7 @@ def run_all(stop_on_fail=False, group=None):
         lambda: check_conv(2, 16, 16, 320, 320, ksize=1, out_fp32=False, scale=0.7),
         lambda: check_temporal_conv(2, 16, 8, 8, 128, 128),
         lambda: check_temporal_conv(1, 14, 16, 16, 320, 320),
+    ], "attn": [
         lambda: check_attention(1, 2, 256, 256, 64),
         lambda: check_attention(2, 5, 1024, 1024, 64),
         lambda: check_attention(2, 10, 1000, 77, 64),
@@ -470,14 +902,15 @@ def run_all(stop_on_fail=False, group=None):
         lambda: check_attention(2, 5, 1024, 1024, 64, ramp=40.0),
         lambda: check_attention(1, 8, 300, 640, 160, ramp=20.0),
         lambda: check_attention(1, 4, 512, 2048, 64, ramp=4.0),
-        # short-KV kernel (Lk <= 80, head dim <= 64): several work items per persistent CTA (ring / phase wrap-around,
-        # deferred output write of the previous item), Lk = 80 / 33 / 1, partial last query tile, padded head dim
+        # a single, partial KV tile (Lk = 77 / 80 / 33 / 1 of 128: the key-tail mask decides every row's softmax, and at
+        # Lk = 1 127 of the 128 keys are masked), grids of up to 2560 CTAs, a partial last query tile, padded head dim
         lambda: check_attention(16, 20, 1024, 77, 64),
         lambda: check_attention(8, 16, 700, 80, 64),
         lambda: check_attention(6, 10, 1280, 33, 40),
         lambda: check_attention(4, 8, 640, 1, 64),
         lambda: check_temporal_attention(2, 16, 64, 5),
         lambda: check_temporal_attention(1, 14, 100, 10),
+    ], "misc": [
         lambda: check_groupnorm(2, 32, 32, 320),
         lambda: check_groupnorm(2, 16, 16, 640, up=True),
         lambda: check_groupnorm(2, 16, 16, 640, c2=320, eps=1e-5),
@@ -511,11 +944,8 @@ def run_all(stop_on_fail=False, group=None):
         check_layout_pool,
         check_router,
         check_cfg,
-    ]
-    groups = {"gemm": (0, 18), "conv": (18, 32), "attn": (32, 49), "misc": (49, len(plan))}
-    if group:
-        lo, hi = groups[group]
-        plan = plan[lo:hi]
+    ], "layouts": [fn for _, fn in LAYOUT_CHECKS]}
+    plan = groups[group] if group else [fn for fns in groups.values() for fn in fns]
     for fn in plan:
         n0 = len(RESULTS)
         try:

@@ -214,9 +214,10 @@ def upsample2x(x):
     return x.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).contiguous()
 
 
-def i2vgen_latent_encoder(x, clips, frames, params):
+def i2vgen_latent_encoder(x, clips, frames, params, *, attn_scale=0.5):
     """x [clips*frames, H, W, Cs] (first 4 channels used); params fp32 [288], layout in include/ctrl_adapter_b200.h:
-    per pixel over the frames of a clip: h = x + to_out(attn(LN(x))) with 2 heads x 4; y = h + W2 gelu(W1 h + b1) + b2."""
+    per pixel over the frames of a clip: h = x + to_out(attn(LN(x))) with 2 heads x 4; y = h + W2 gelu(W1 h + b1) + b2.
+    attn_scale: 4^-0.5 (head dim 4); other values only model a wrong kernel in tests/test_kernel_checks_cpu.py."""
     n, h, w_, cs = x.shape
     p = params.float()
     o = 0
@@ -236,7 +237,7 @@ def i2vgen_latent_encoder(x, clips, frames, params):
     def heads(t):
         return t.reshape(*t.shape[:-1], 2, 4).transpose(-2, -3)  # [clip, pixel, head, frame, 4]
     q, k, v = (heads(_r(xn @ m.t())) for m in (wq, wk, wv))
-    a = _r(torch.softmax(q @ k.transpose(-1, -2) * 0.5, dim=-1) @ v)
+    a = _r(torch.softmax(q @ k.transpose(-1, -2) * attn_scale, dim=-1) @ v)
     a = a.transpose(-2, -3).reshape(clips, h * w_, frames, 8)
     hcur = _r(_r(a @ wo.t() + bo) + xs)
     y = _r(_r(_r(F.gelu(_r(hcur @ w1.t() + b1))) @ w2.t() + b2) + hcur)

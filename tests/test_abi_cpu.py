@@ -56,6 +56,23 @@ def test_fails_loudly_without_gpu(lib):
     assert len(lib.ca_last_error()) > 0
 
 
+def test_gemm_rejects_blend_with_fp32_output(lib):
+    """The fp32 epilogue has no AlphaBlender term: ca_gemm refuses the combination instead of dropping the blend.
+    Argument validation runs before any tensor map is encoded, so placeholder pointers and no device suffice."""
+    from ctrl_adapter_b200 import _lib
+    d = _lib.GemmDesc()
+    d.nsrc, d.ntaps = 1, 1
+    d.box[0], d.box[1], d.box[2], d.box[3] = 128, 1, 1, 1
+    d.a[0] = d.w = d.out = d.blend_src = d.blend_alpha = 256  # never dereferenced
+    d.a_channels[0] = d.a_c_len[0] = d.w_k_per_tap = 64
+    d.a_dims[0] = d.a_dims[1] = d.a_dims[2] = d.a_dims[3] = 1
+    d.out_dims[0] = d.out_dims[1] = d.out_dims[2] = d.out_dims[3] = 1
+    d.w_rows = d.n_out = 64
+    d.out_fp32 = 1
+    assert lib.ca_gemm(ctypes.byref(d), None) == 3  # CA_ERR_UNSUPPORTED
+    assert b"blend" in lib.ca_last_error()
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "ctrl_adapter_b200")
     for f in os.listdir(pkg):
