@@ -2,11 +2,17 @@
 // UNets: wgmma tensor-core MMAs, TMA-fed 128B-swizzled shared memory, online softmax in registers.
 //
 // One CTA = 128 query rows of one (batch, head) and one 64-wide slice of the value head dim; 384 threads:
-//   warpgroup 0, one thread: TMA producer (Q once, then K and V tiles of 128 keys through a 2-stage ring)
-//   warpgroups 1, 2        : 64 query rows each.  Per KV tile: S = Q K^T (m64n128, K = 64 * DQ, both operands K-major
-//                            in shared memory) into registers; online softmax (exp2, running max and row sum in fp32);
-//                            P is rounded to bf16 and fed from registers as the A operand of O += P V (m64n64, V read
-//                            MN-major from shared memory).  The ring slot is released once both wgmma have retired.
+//   warpgroup 0, one thread: TMA producer.  Q once, then per tile of 128 keys the K chunks and then the V slice, each
+//                            through its own ring of kStages slots (full / empty mbarrier pair per slot), so that
+//                            Q K^T waits only for K.
+//   warpgroups 1, 2        : 64 query rows each.  S = Q K^T (m64n128, K = 64 * DQ, both operands K-major in shared
+//                            memory) into registers; online softmax (exp2, running max and row sum in fp32); P is
+//                            rounded to bf16 and fed from registers as the A operand of O += P V (m64n64, V read
+//                            MN-major from shared memory).
+// Schedule of one consumer warpgroup: Q K_{j+1}^T and P_j V_j are issued back to back, and the softmax of S_{j+1} runs
+// while P_j V_j is still on the tensor cores; O is rescaled by the new tile's correction once P_j V_j has retired.  The
+// two warpgroups take turns issuing (named barriers), so one's softmax overlaps the other's MMAs.  The arithmetic and
+// its order are those of a plain tile-by-tile loop: only the schedule overlaps.
 // Epilogue: O / l, one bf16 rounding, 4-byte stores.  Head dims 128 / 192 (the zero-padded ControlNet heads) use
 // DQ = 2 / 3 chunks of 64 for Q K^T.
 #include "common.cuh"
@@ -22,12 +28,22 @@ static constexpr uint32_t kChunkBytes = 128 * 64 * 2;  // one [128 rows x 64 col
 
 template <int DQ>
 struct AttnCfg {
-  static constexpr int kStages = 2;
   static constexpr uint32_t kQBytes = DQ * kChunkBytes;
-  static constexpr uint32_t kStageBytes = (DQ + 1) * kChunkBytes;  // K chunks + one V slice
-  static constexpr uint32_t kDataBytes = kQBytes + kStages * kStageBytes;
+  static constexpr uint32_t kKBytes = DQ * kChunkBytes;  // one K slot: DQ chunks
+  static constexpr uint32_t kVBytes = kChunkBytes;       // one V slot: one 64-wide slice
+  // 227 KB per block on H100, minus Q, alignment slack and barriers: 4 stages at DQ 1 / 2, 2 at DQ 3
+  static constexpr uint32_t kBudget = 232448 - kQBytes - 1024 - 256;
+  static constexpr int kStagesRaw = kBudget / (kKBytes + kVBytes);
+  static constexpr int kStages = kStagesRaw > 4 ? 4 : kStagesRaw;
+  static constexpr uint32_t kDataBytes = kQBytes + kStages * (kKBytes + kVBytes);
   static constexpr uint32_t kSmemBytes = kDataBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kStages >= 2, "the K / V rings need two slots");
+  static_assert((1 + 4 * kStages) * 8 <= 256, "barrier area");
 };
+
+// named barriers of the two consumer warpgroups' issue turns (barrier 1 + w: warpgroup w may issue)
+static constexpr int kTurnBar = 1;
+static constexpr int kTurnThreads = 256;
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -35,21 +51,63 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
+// Online softmax of one S tile in place (s becomes the unrounded P), updating the running max / sum; corr = the factor
+// O must be scaled by before this tile's P V.  Thread holds rows (r, r + 8) x key columns 8 jj + 2 tig + {0, 1}.
+// kMask: keys past kv_valid are set to -inf (only the last KV tile can have them).
+template <bool kMask>
+__device__ __forceinline__ void online_softmax(float (&s)[64], float scale_log2, int kv_valid, int tig,
+                                               float (&m_run)[2], float (&l_run)[2], float (&corr)[2]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int col = 8 * jj + 2 * tig + (e & 1);
+      float x = s[4 * jj + e] * scale_log2;
+      if (kMask && col >= kv_valid) x = -INFINITY;
+      s[4 * jj + e] = x;
+      mx[e >> 1] = fmaxf(mx[e >> 1], x);
+    }
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    const float m_new = fmaxf(m_run[hh], mx[hh]);
+    corr[hh] = fast_exp2(m_run[hh] - m_new);  // 0 on the first tile (m_run = -inf)
+    m_run[hh] = m_new;
+    l_run[hh] *= corr[hh];
+  }
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float pv = fast_exp2(s[4 * jj + e] - m_run[e >> 1]);
+      s[4 * jj + e] = pv;
+      l_run[e >> 1] += pv;
+    }
+  }
+}
+
 template <int DQ>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
   using Cfg = AttnCfg<DQ>;
+  constexpr uint32_t S = Cfg::kStages;
   CA_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* smem_q = smem;
-  uint8_t* smem_kv = smem + Cfg::kQBytes;
+  uint8_t* smem_k = smem + Cfg::kQBytes;            // [kStages] x kKBytes
+  uint8_t* smem_v = smem_k + S * Cfg::kKBytes;      // [kStages] x kVBytes
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kDataBytes);
   uint64_t* q_full = bars;
-  uint64_t* full = bars + 1;   // [kStages]
-  uint64_t* empty = bars + 3;  // [kStages]
+  uint64_t* k_full = bars + 1;           // [kStages]
+  uint64_t* k_empty = bars + 1 + S;      // [kStages]
+  uint64_t* v_full = bars + 1 + 2 * S;   // [kStages]
+  uint64_t* v_empty = bars + 1 + 3 * S;  // [kStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -65,9 +123,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
     mbar_init(q_full, 1);
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);  // one arrive per consumer warp
+    for (uint32_t s = 0; s < S; ++s) {
+      mbar_init(&k_full[s], 1);
+      mbar_init(&k_empty[s], 8);  // one arrive per consumer warp
+      mbar_init(&v_full[s], 1);
+      mbar_init(&v_empty[s], 8);
     }
     fence_mbar_init();
   }
@@ -81,16 +141,17 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       const int kvb = b / p.kv_batch_div;
       mbar_arrive_expect_tx(q_full, Cfg::kQBytes);
       for (int c = 0; c < DQ; ++c) tma_load_3d(smem_q + c * kChunkBytes, &tmap_q, q_full, h * dpad + c * 64, q0, b);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < nkv; ++j) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t* dst = smem_kv + stage * Cfg::kStageBytes;
-        mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
+      for (uint32_t j = 0; j < static_cast<uint32_t>(nkv); ++j) {
+        const uint32_t slot = j % S;
+        const uint32_t phase = (j / S) & 1u;
+        mbar_wait(&k_empty[slot], phase ^ 1);
+        uint8_t* kdst = smem_k + slot * Cfg::kKBytes;
+        mbar_arrive_expect_tx(&k_full[slot], Cfg::kKBytes);
         for (int c = 0; c < DQ; ++c)
-          tma_load_3d(dst + c * kChunkBytes, &tmap_k, &full[stage], h * dpad + c * 64, j * kTileKV, kvb);
-        tma_load_3d(dst + DQ * kChunkBytes, &tmap_v, &full[stage], h * dpad + vs * 64, j * kTileKV, kvb);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          tma_load_3d(kdst + c * kChunkBytes, &tmap_k, &k_full[slot], h * dpad + c * 64, j * kTileKV, kvb);
+        mbar_wait(&v_empty[slot], phase ^ 1);
+        mbar_arrive_expect_tx(&v_full[slot], Cfg::kVBytes);
+        tma_load_3d(smem_v + slot * Cfg::kVBytes, &tmap_v, &v_full[slot], h * dpad + vs * 64, j * kTileKV, kvb);
       }
     }
     return;
@@ -106,62 +167,38 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY};
   float l_run[2] = {0.f, 0.f};
+  float corr[2];
+  float s[64];
+  uint32_t pa[8][4];
   const uint32_t q_addr = smem_u32(smem_q) + cw * 64 * 128;
-  mbar_wait(q_full, 0);
+  const int last = nkv - 1;
+  const int kv_valid_last = p.lk - last * kTileKV;
 
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int j = 0; j < nkv; ++j) {
-    mbar_wait(&full[stage], phase);
-    const uint32_t kv_addr = smem_u32(smem_kv + stage * Cfg::kStageBytes);
-    float s[64];
-    wgmma_fence();
+  // S = Q K_j^T (one commit group; K_j has landed)
+  auto issue_qk = [&](uint32_t j) {
+    const uint32_t k_addr = smem_u32(smem_k + (j % S) * Cfg::kKBytes);
 #pragma unroll
     for (int c = 0; c < DQ; ++c) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         Wgmma<128>::ss(s, gmma_desc_sw128(q_addr + c * kChunkBytes + k * 32, 16, 1024),
-                       gmma_desc_sw128(kv_addr + c * kChunkBytes + k * 32, 16, 1024), (c | k) != 0 ? 1 : 0);
+                       gmma_desc_sw128(k_addr + c * kChunkBytes + k * 32, 16, 1024), (c | k) != 0 ? 1 : 0);
       }
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-
-    // ---- online softmax: thread holds rows (r, r + 8) x key columns 8 jj + 2 tig + {0, 1} ----
-    const int kv_valid = min(kTileKV, p.lk - j * kTileKV);
-    float mx[2] = {-INFINITY, -INFINITY};
+  };
+  // O += P V_j (one commit group; V_j has landed)
+  auto issue_pv = [&](uint32_t j) {
+    const uint32_t v_addr = smem_u32(smem_v + (j % S) * Cfg::kVBytes);
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int col = 8 * jj + 2 * tig + (e & 1);
-        float x = s[4 * jj + e] * p.scale_log2;
-        if (col >= kv_valid) x = -INFINITY;
-        s[4 * jj + e] = x;
-        mx[e >> 1] = fmaxf(mx[e >> 1], x);
-      }
-    }
-    float corr[2];
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      const float m_new = fmaxf(m_run[hh], mx[hh]);
-      corr[hh] = fast_exp2(m_run[hh] - m_new);  // 0 on the first tile (m_run = -inf)
-      m_run[hh] = m_new;
-      l_run[hh] *= corr[hh];
-    }
-    uint32_t pa[8][4];
-#pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float pv = fast_exp2(s[4 * jj + e] - m_run[e >> 1]);
-        s[4 * jj + e] = pv;
-        l_run[e >> 1] += pv;
-      }
-    }
+    for (int kk = 0; kk < 8; ++kk) Wgmma<64>::rs_bt(o, pa[kk], gmma_desc_sw128(v_addr + kk * 2048, 8192, 1024), 1);
+    wgmma_commit();
+  };
+  auto softmax = [&](int j) {
+    if (j == last) online_softmax<true>(s, p.scale_log2, kv_valid_last, tig, m_run, l_run, corr);
+    else online_softmax<false>(s, p.scale_log2, kTileKV, tig, m_run, l_run, corr);
+  };
+  auto pack_p = [&]() {
 #pragma unroll
     for (int kk = 0; kk < 8; ++kk) {
       pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
@@ -169,20 +206,66 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
       pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
     }
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] *= corr[(i >> 1) & 1];
+  };
+  // Issue turns alternate between the warpgroups, nkv + 1 per warpgroup (S_0; S_{j+1} with P_j V_j; the last P V).
+  // Warpgroup 0 needs no go-ahead for its first turn and warpgroup 1 gives none after its last, so every arrive is
+  // matched by exactly one sync.
+  auto turn_begin = [&](bool first) {
+    if (!(first && cw == 0)) named_bar_sync(kTurnBar + cw, kTurnThreads);
+  };
+  auto turn_end = [&](bool final_turn) {
+    if (!(final_turn && cw == 1)) named_bar_arrive(kTurnBar + (cw ^ 1), kTurnThreads);
+  };
+  auto wait_full = [&](uint64_t* full, uint32_t j) { mbar_wait(&full[j % S], (j / S) & 1u); };
+  auto release = [&](uint64_t* empty, uint32_t j) {
+    if (lane == 0) mbar_arrive(&empty[j % S]);
+  };
 
-    // ---- O += P V ----
-    const uint32_t v_addr = kv_addr + DQ * kChunkBytes;
+  mbar_wait(q_full, 0);
+
+  // prologue: S_0 and its softmax (O is still 0: no rescale)
+  wait_full(k_full, 0);
+  turn_begin(true);
+  wgmma_fence();
+  issue_qk(0);
+  turn_end(false);
+  wgmma_wait<0>();
+  reg_fence(s);
+  release(k_empty, 0);
+  softmax(0);
+  pack_p();
+
+  // steady state: S_{j+1} and P_j V_j in flight together; the softmax of S_{j+1} overlaps P_j V_j
+  for (int j = 0; j < last; ++j) {
+    wait_full(k_full, j + 1);
+    wait_full(v_full, j);
+    turn_begin(false);
     wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) Wgmma<64>::rs_bt(o, pa[kk], gmma_desc_sw128(v_addr + kk * 2048, 8192, 1024), 1);
-    wgmma_commit();
+    issue_qk(j + 1);
+    issue_pv(j);
+    turn_end(false);
+    wgmma_wait<1>();
+    reg_fence(s);
+    release(k_empty, j + 1);
+    softmax(j + 1);
+    reg_fence(s);
     wgmma_wait<0>();
     reg_fence(o);
-    if (lane == 0) mbar_arrive(&empty[stage]);
-    if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    release(v_empty, j);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= corr[(i >> 1) & 1];
+    pack_p();
   }
+
+  // tail: the last P V
+  wait_full(v_full, last);
+  turn_begin(false);
+  wgmma_fence();
+  issue_pv(last);
+  turn_end(true);
+  wgmma_wait<0>();
+  reg_fence(o);
+  release(v_empty, last);
 
   // ---- epilogue: O / l ----
 #pragma unroll
