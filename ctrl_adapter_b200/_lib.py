@@ -109,8 +109,7 @@ def load():
         raise CtrlAdapterB200Error(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(there is no CPU / PyTorch fallback for the hot path)")
-    # CA_B200_LIB: developer override (another build of the library, e.g. -DCA_NO_PDL)
-    lib = C.CDLL(os.environ.get("CA_B200_LIB", LIB_PATH))
+    lib = C.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol
         fn.argtypes = argtypes

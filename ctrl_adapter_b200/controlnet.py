@@ -6,7 +6,6 @@ Same constructor kwargs (default SD1.5 topology), forward signature (including t
 """
 from __future__ import annotations
 
-import os
 from typing import List, Optional, Tuple, Union
 
 import torch
@@ -33,14 +32,12 @@ class ControlNetConditioningEmbedding(nn.Module):
         self.conv_out = Conv2d(block_out_channels[-1], out_channels, 3)
 
     # the 8- / 16- / 32-channel stride-1 convolutions at full image resolution run with 8 / 4 / 2 adjacent pixels folded
-    # into the channel axis (layers.Conv2d.forward_folded) instead of padding every tap to 64 channels; GPU-verified in
-    # round 2 (checked by the GPU test group `fold`).  CA_FOLD_SMALL_CONV=0 restores the padded form.
+    # into the channel axis (layers.Conv2d.forward_folded) instead of padding every tap to 64 channels; the GPU test
+    # group `fold` checks the folded form against the padded one
     def forward(self, cond_nhwc8):
-        fold = os.environ.get("CA_FOLD_SMALL_CONV", "1") != "0"
-        conv = (lambda m, x, **kw: m.forward_folded(x, **kw)) if fold else (lambda m, x, **kw: m(x, **kw))
-        e = conv(self.conv_in, cond_nhwc8, act=ACT_SILU)
+        e = self.conv_in.forward_folded(cond_nhwc8, act=ACT_SILU)
         for blk in self.blocks:
-            e = conv(blk, e, act=ACT_SILU) if blk.stride == 1 else blk(e, act=ACT_SILU)
+            e = blk.forward_folded(e, act=ACT_SILU) if blk.stride == 1 else blk(e, act=ACT_SILU)
         return self.conv_out(e)
 
 

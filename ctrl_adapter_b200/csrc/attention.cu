@@ -26,6 +26,16 @@ static constexpr int kTileKV = 128;
 static constexpr int kAttnThreads = 384;
 static constexpr uint32_t kChunkBytes = 128 * 64 * 2;  // one [128 rows x 64 cols] bf16 swizzle tile = 16 KB
 
+struct AttnParams {
+  int batch, heads, lq, lk;
+  int kv_batch_div;    // K/V batch index = query batch index / kv_batch_div (context shared by the frames of a clip)
+  int dqk_chunks;      // padded head dim / 64 used for QK^T
+  int v_slices;        // padded head dim / 64 (PV is computed one 64-wide slice per CTA)
+  float scale_log2;    // softmax scale * log2(e)
+  __nv_bfloat16* out;  // [batch, lq, heads * 64 * v_slices]
+  long long out_batch_stride, out_row_stride;  // elements
+};
+
 template <int DQ>
 struct AttnCfg {
   static constexpr uint32_t kQBytes = DQ * kChunkBytes;
@@ -299,18 +309,48 @@ static cudaError_t launch_dq(const CUtensorMap& q, const CUtensorMap& k, const C
     attr_set = true;
   }
   const dim3 grid((p.lq + kTileQ - 1) / kTileQ, p.heads * p.v_slices, p.batch);
-  CA_KERNEL_LAUNCH(kern, grid, kAttnThreads, Cfg::kSmemBytes, stream, q, k, v, p);
-  return cudaGetLastError();
+  return launch_pdl(kern, grid, kAttnThreads, Cfg::kSmemBytes, stream, q, k, v, p);
 }
 
-cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p,
-                             cudaStream_t stream) {
-  switch (p.dqk_chunks) {
-    case 1: return launch_dq<1>(q, k, v, p, stream);
-    case 2: return launch_dq<2>(q, k, v, p, stream);
-    case 3: return launch_dq<3>(q, k, v, p, stream);
-    default: return cudaErrorInvalidValue;
+extern "C" int ca_attention(const ca_attention_desc* d, void* cuda_stream) {
+  if (!d) return fail(CA_ERR_INVALID, "null desc");
+  cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+  if (d->head_dim_pad != 64 && d->head_dim_pad != 128 && d->head_dim_pad != 192)
+    return fail(CA_ERR_UNSUPPORTED, "head_dim_pad must be 64, 128 or 192 (got %d)", d->head_dim_pad);
+  if (d->batch < 1 || d->heads < 1 || d->lq < 1 || d->lk < 1) return fail(CA_ERR_INVALID, "empty attention problem");
+  const int kv_div = d->kv_batch_div > 0 ? d->kv_batch_div : 1;
+  if (d->batch % kv_div != 0) return fail(CA_ERR_INVALID, "batch must be a multiple of kv_batch_div");
+  const cuuint64_t ctot = static_cast<cuuint64_t>(d->heads) * d->head_dim_pad;
+  CUtensorMap tq, tk, tv;
+  const cuuint32_t box[3] = {64, 128, 1};
+  {
+    cuuint64_t dims[3] = {ctot, (cuuint64_t)d->lq, (cuuint64_t)d->batch};
+    cuuint64_t st[2] = {(cuuint64_t)d->q_row_stride * 2, (cuuint64_t)d->q_batch_stride * 2};
+    int rc = make_tmap(&tq, d->q, 3, dims, st, box);
+    if (rc) return rc;
   }
+  {
+    cuuint64_t dims[3] = {ctot, (cuuint64_t)d->lk, (cuuint64_t)(d->batch / kv_div)};
+    cuuint64_t st[2] = {(cuuint64_t)d->k_row_stride * 2, (cuuint64_t)d->k_batch_stride * 2};
+    int rc = make_tmap(&tk, d->k, 3, dims, st, box);
+    if (rc) return rc;
+    cuuint64_t sv[2] = {(cuuint64_t)d->v_row_stride * 2, (cuuint64_t)d->v_batch_stride * 2};
+    rc = make_tmap(&tv, d->v, 3, dims, sv, box);
+    if (rc) return rc;
+  }
+  AttnParams p;
+  p.batch = d->batch; p.heads = d->heads; p.lq = d->lq; p.lk = d->lk;
+  p.kv_batch_div = kv_div;
+  p.dqk_chunks = d->head_dim_pad / 64;
+  p.v_slices = d->head_dim_pad / 64;
+  p.scale_log2 = d->scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(d->out);
+  p.out_batch_stride = d->out_batch_stride;
+  p.out_row_stride = d->out_row_stride;
+  const cudaError_t e = p.dqk_chunks == 1   ? launch_dq<1>(tq, tk, tv, p, stream)
+                        : p.dqk_chunks == 2 ? launch_dq<2>(tq, tk, tv, p, stream)
+                                            : launch_dq<3>(tq, tk, tv, p, stream);
+  return launched(e, "attention launch");
 }
 
 }  // namespace ca

@@ -40,52 +40,8 @@ __device__ __forceinline__ uint32_t add_bf16x2(uint32_t a, uint32_t b) {
   asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
   return d;
 }
-__device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
 __device__ __forceinline__ float bf16lo_to_float(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16hi_to_float(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-
-// ---- fp32 pairs kept in one 64-bit value (per-lane IEEE fma / add / mul, round to nearest) ----
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  float a0, a1, b0, b1, c0, c1;
-  unpack_f32x2(a, a0, a1);
-  unpack_f32x2(b, b0, b1);
-  unpack_f32x2(c, c0, c1);
-  return pack_f32x2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  float a0, a1, b0, b1;
-  unpack_f32x2(a, a0, a1);
-  unpack_f32x2(b, b0, b1);
-  return pack_f32x2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
-}
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  float a0, a1, b0, b1;
-  unpack_f32x2(a, a0, a1);
-  unpack_f32x2(b, b0, b1);
-  return pack_f32x2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ----------------------------------------------------------------------------
 // mbarrier
@@ -169,12 +125,6 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// 16-byte asynchronous global -> shared copy (LDGSTS)
-__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-
 // ----------------------------------------------------------------------------
 // wgmma (Hopper warpgroup MMA): fences, commit / wait, shared-memory matrix descriptor
 // ----------------------------------------------------------------------------
@@ -221,17 +171,17 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 }  // namespace ca
 
 // ---------------------------------------------------------------------------------------------------------------
-// Programmatic dependent launch (-DCA_NO_PDL builds without it).
+// Programmatic dependent launch.
 // With ~1500 launches per step, every kernel's prologue (barrier init, descriptor prefetch) and the
 // launch latency itself sit between the tail of one kernel and the first useful cycle of the next.  With PDL each
 // kernel (a) tells the scheduler right away that its dependents may be launched as SMs free up and (b) waits for the
 // previous grid's completion only after its own prologue, before the first global-memory access.  Without the launch
-// attribute both instructions are no-ops, and with -DCA_NO_PDL neither is emitted.
+// attribute both instructions are no-ops.
 // ---------------------------------------------------------------------------------------------------------------
-#ifndef CA_NO_PDL
 #define CA_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;")
 #define CA_PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
 namespace ca {
+// every kernel of the library is launched through this: returns the status of cudaLaunchKernelEx
 template <typename K, typename... A>
 inline cudaError_t launch_pdl(K kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A... args) {
   cudaLaunchConfig_t cfg = {};
@@ -247,31 +197,3 @@ inline cudaError_t launch_pdl(K kernel, dim3 grid, dim3 block, size_t smem, cuda
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 }  // namespace ca
-// `kernel` must be a plain identifier or a function pointer variable (no template commas inside the macro argument)
-#define CA_KERNEL_LAUNCH(kernel, grid, block, smem, stream, ...) \
-  (void)ca::launch_pdl(kernel, dim3(grid), dim3(block), smem, stream, __VA_ARGS__)
-#else
-#define CA_PDL_TRIGGER()
-#define CA_PDL_WAIT()
-#define CA_KERNEL_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
-#endif
-
-// Developer instrumentation: cycles each role of a kernel spends blocked, 16 counters per CTA
-// written through the `trace` pointer of the kernel's Params struct.  Compiled out unless -DCA_TRACE.
-#ifdef CA_TRACE
-#define TR_CTA() (blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z))
-#define TR_DECL(v_) long long v_ = 0
-#define TR_WAIT(v_, stmt) do { const long long _t0 = clock64(); stmt; v_ += clock64() - _t0; } while (0)
-#define TR_PUT(slot, v_) do { if (p.trace != nullptr && TR_CTA() < 4096) p.trace[TR_CTA() * 16 + (slot)] = static_cast<unsigned long long>(v_); } while (0)
-#define TR_NOW() clock64()
-// event log of CTA 0 (behind the per-CTA counters): (event id, clock) pairs, first 96 events of each logging thread
-#define TR_EVT_DECL(base_) int _evt_n = 0; const int _evt_base = (base_)
-#define TR_EVT(id_) do { if (p.trace != nullptr && TR_CTA() == 0 && _evt_n < 96) { p.trace[16 * 4096 + (_evt_base + _evt_n) * 2] = (id_); p.trace[16 * 4096 + (_evt_base + _evt_n) * 2 + 1] = static_cast<unsigned long long>(clock64()); ++_evt_n; } } while (0)
-#else
-#define TR_DECL(v_)
-#define TR_WAIT(v_, stmt) stmt
-#define TR_PUT(slot, v_)
-#define TR_NOW() 0
-#define TR_EVT_DECL(base_)
-#define TR_EVT(id_)
-#endif

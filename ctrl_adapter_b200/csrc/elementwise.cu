@@ -1,6 +1,7 @@
-// Small HBM-bound kernels of the denoising step: timestep sinusoid, layout changes at the module boundary,
-// pooling / up-sampling, router softmax + weighted merge, CFG + scheduler update, temporal (frame-axis)
-// attention.  All vectorised to 16-byte accesses where the layout allows.
+// Small HBM-bound kernels of the denoising step and their entry points: timestep sinusoid, layout changes at the
+// module boundary, pooling / up-sampling, router softmax + weighted merge, CFG + scheduler update, the I2VGen-XL latent
+// encoder, the SVD decoder's frame convolution and the VAE's row softmax.  All vectorised to 16-byte accesses where the
+// layout allows.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -36,12 +37,12 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, int n, in
     if ((dim & 1) && k == 0) o[dim - 1] = __float2bfloat16_rn(0.f);
   }
 }
-cudaError_t launch_timestep_embedding(const float* t, int n, int dim, int flip_sin_to_cos, float freq_shift,
-                                      int round_t_bf16, __nv_bfloat16* out, cudaStream_t stream) {
+extern "C" int ca_timestep_embedding(const float* t, int32_t n, int32_t dim, int32_t flip_sin_to_cos, float freq_shift,
+                                     int32_t round_t_bf16, void* out, void* s) {
   const long long total = static_cast<long long>(n) * (dim / 2);
-  CA_KERNEL_LAUNCH(timestep_embedding_kernel, blocks_for(total, 256), 256, 0, stream, t, n, dim, flip_sin_to_cos, freq_shift,
-                                                                        round_t_bf16, out);
-  return cudaGetLastError();
+  return launched(launch_pdl(timestep_embedding_kernel, blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(s), t,
+                             n, dim, flip_sin_to_cos, freq_shift, round_t_bf16, static_cast<__nv_bfloat16*>(out)),
+                  "timestep_embedding");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -60,11 +61,11 @@ __global__ void silu_kernel(const uint4* __restrict__ x, long long nvec, uint4* 
     y[i] = make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
   }
 }
-cudaError_t launch_silu(const __nv_bfloat16* x, long long n, __nv_bfloat16* y, cudaStream_t stream) {
-  if (n & 7) return cudaErrorInvalidValue;
-  CA_KERNEL_LAUNCH(silu_kernel, blocks_for(n / 8, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), n / 8,
-                                                          reinterpret_cast<uint4*>(y));
-  return cudaGetLastError();
+extern "C" int ca_silu(const void* x, int64_t n, void* y, void* s) {
+  if (n & 7) return fail(CA_ERR_INVALID, "silu: n (%lld) must be a multiple of 8", (long long)n);
+  return launched(launch_pdl(silu_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const uint4*>(x), n / 8, static_cast<uint4*>(y)),
+                  "silu");
 }
 __global__ void add_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, long long nvec,
                            uint4* __restrict__ y) {
@@ -85,13 +86,11 @@ __global__ void add_kernel(const uint4* __restrict__ a, const uint4* __restrict_
     y[i] = o;
   }
 }
-cudaError_t launch_add(const __nv_bfloat16* a, const __nv_bfloat16* b, long long n, __nv_bfloat16* y,
-                       cudaStream_t stream) {
-  if (n & 7) return cudaErrorInvalidValue;
-  CA_KERNEL_LAUNCH(add_kernel, blocks_for(n / 8, 256), 256, 0, stream, reinterpret_cast<const uint4*>(a),
-                                                         reinterpret_cast<const uint4*>(b), n / 8,
-                                                         reinterpret_cast<uint4*>(y));
-  return cudaGetLastError();
+extern "C" int ca_add(const void* a, const void* b, int64_t n, void* y, void* s) {
+  if (n & 7) return fail(CA_ERR_INVALID, "add: n (%lld) must be a multiple of 8", (long long)n);
+  return launched(launch_pdl(add_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const uint4*>(a), static_cast<const uint4*>(b), n / 8, static_cast<uint4*>(y)),
+                  "add");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -120,12 +119,16 @@ __global__ void nchw_to_nhwc_kernel(const SrcT* __restrict__ x, int c, long long
     if (p < hw && ch < c_pad) y[(static_cast<long long>(n) * hw + p) * c_pad + ch] = __float2bfloat16_rn(tile[threadIdx.x][i]);
   }
 }
-cudaError_t launch_nchw_to_nhwc(const void* x, int src_fp32, int n, int c, long long hw, int c_pad, __nv_bfloat16* y,
-                                cudaStream_t stream) {
-  dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c_pad + 31) / 32, n), block(32, 8);
-  if (src_fp32) CA_KERNEL_LAUNCH(nchw_to_nhwc_kernel<float>, grid, block, 0, stream, static_cast<const float*>(x), c, hw, c_pad, y);
-  else CA_KERNEL_LAUNCH(nchw_to_nhwc_kernel<__nv_bfloat16>, grid, block, 0, stream, static_cast<const __nv_bfloat16*>(x), c, hw, c_pad, y);
-  return cudaGetLastError();
+extern "C" int ca_nchw_to_nhwc(const void* x, int32_t src_fp32, int32_t n, int32_t c, int64_t hw, int32_t c_pad,
+                               void* y_, void* s) {
+  const dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c_pad + 31) / 32, n), block(32, 8);
+  cudaStream_t stream = static_cast<cudaStream_t>(s);
+  __nv_bfloat16* y = static_cast<__nv_bfloat16*>(y_);
+  const cudaError_t e =
+      src_fp32 ? launch_pdl(nchw_to_nhwc_kernel<float>, grid, block, 0, stream, static_cast<const float*>(x), c, hw, c_pad, y)
+               : launch_pdl(nchw_to_nhwc_kernel<__nv_bfloat16>, grid, block, 0, stream,
+                            static_cast<const __nv_bfloat16*>(x), c, hw, c_pad, y);
+  return launched(e, "nchw_to_nhwc");
 }
 template <typename DstT>
 __global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ x, int c, int c_stride, long long hw,
@@ -150,12 +153,16 @@ __global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ x, int c, 
     if (ch < c && p < hw) y[(static_cast<long long>(n) * c + ch) * hw + p] = static_cast<DstT>(tile[threadIdx.x][i]);
   }
 }
-cudaError_t launch_nhwc_to_nchw(const __nv_bfloat16* x, int n, int c, int c_stride, long long hw, void* y,
-                                int dst_fp32, cudaStream_t stream) {
-  dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c + 31) / 32, n), block(32, 8);
-  if (dst_fp32) CA_KERNEL_LAUNCH(nhwc_to_nchw_kernel<float>, grid, block, 0, stream, x, c, c_stride, hw, static_cast<float*>(y));
-  else CA_KERNEL_LAUNCH(nhwc_to_nchw_kernel<__nv_bfloat16>, grid, block, 0, stream, x, c, c_stride, hw, static_cast<__nv_bfloat16*>(y));
-  return cudaGetLastError();
+extern "C" int ca_nhwc_to_nchw(const void* x_, int32_t n, int32_t c, int32_t c_stride, int64_t hw, void* y,
+                               int32_t dst_fp32, void* s) {
+  const dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c + 31) / 32, n), block(32, 8);
+  cudaStream_t stream = static_cast<cudaStream_t>(s);
+  const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(x_);
+  const cudaError_t e =
+      dst_fp32 ? launch_pdl(nhwc_to_nchw_kernel<float>, grid, block, 0, stream, x, c, c_stride, hw, static_cast<float*>(y))
+               : launch_pdl(nhwc_to_nchw_kernel<__nv_bfloat16>, grid, block, 0, stream, x, c, c_stride, hw,
+                            static_cast<__nv_bfloat16*>(y));
+  return launched(e, "nhwc_to_nchw");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -181,12 +188,14 @@ __global__ void avgpool_kernel(const __nv_bfloat16* __restrict__ x, int h, int w
     y[i] = __float2bfloat16_rn(acc * inv);
   }
 }
-cudaError_t launch_avgpool(const __nv_bfloat16* x, int n, int h, int w, int c, int oh, int ow, __nv_bfloat16* y,
-                           cudaStream_t stream) {
-  if (h % oh != 0 || w % ow != 0) return cudaErrorInvalidValue;
+extern "C" int ca_avgpool(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, int32_t oh, int32_t ow, void* y,
+                          void* s) {
+  if (oh < 1 || ow < 1 || h % oh != 0 || w % ow != 0)
+    return fail(CA_ERR_INVALID, "avgpool: h, w (%d, %d) must be positive multiples of oh, ow (%d, %d)", h, w, oh, ow);
   const long long total = static_cast<long long>(n) * oh * ow * c;
-  CA_KERNEL_LAUNCH(avgpool_kernel, blocks_for(total, 256), 256, 0, stream, x, h, w, c, oh, ow, total, y);
-  return cudaGetLastError();
+  return launched(launch_pdl(avgpool_kernel, blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const __nv_bfloat16*>(x), h, w, c, oh, ow, total, static_cast<__nv_bfloat16*>(y)),
+                  "avgpool");
 }
 
 __global__ void upsample2x_kernel(const uint4* __restrict__ x, int h, int w, int nvec, long long total,
@@ -206,13 +215,12 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, int h, int w, int
     dst[0] = u; dst[nvec] = u; dst[ow * nvec] = u; dst[ow * nvec + nvec] = u;
   }
 }
-cudaError_t launch_upsample2x(const __nv_bfloat16* x, int n, int h, int w, int c, __nv_bfloat16* y,
-                              cudaStream_t stream) {
-  if (c & 7) return cudaErrorInvalidValue;
+extern "C" int ca_upsample2x(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, void* y, void* s) {
+  if (c & 7) return fail(CA_ERR_INVALID, "upsample2x: c (%d) must be a multiple of 8", c);
   const long long total = static_cast<long long>(n) * h * w * (c / 8);
-  CA_KERNEL_LAUNCH(upsample2x_kernel, blocks_for(total, 256), 256, 0, stream, reinterpret_cast<const uint4*>(x), h, w, c / 8, total,
-                                                                reinterpret_cast<uint4*>(y));
-  return cudaGetLastError();
+  return launched(launch_pdl(upsample2x_kernel, blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const uint4*>(x), h, w, c / 8, total, static_cast<uint4*>(y)),
+                  "upsample2x");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -239,15 +247,17 @@ __global__ void router_weights_kernel(const float* __restrict__ logits, const un
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane < nexperts) weights[r * nexperts + lane] = e / s;
 }
-cudaError_t launch_router_weights(const float* logits, const unsigned char* mask, int nrouters, int nexperts,
-                                  float* weights, cudaStream_t stream) {
-  if (nexperts > 32 || nexperts < 1) return cudaErrorInvalidValue;
+extern "C" int ca_router_weights(const float* logits, const uint8_t* mask, int32_t nrouters, int32_t nexperts,
+                                 float* weights, void* s) {
+  if (nexperts < 1 || nexperts > 32) return fail(CA_ERR_INVALID, "router_weights: nexperts must be 1..32 (got %d)", nexperts);
   const int wpb = 4;
-  CA_KERNEL_LAUNCH(router_weights_kernel, (nrouters + wpb - 1) / wpb, wpb * 32, 0, stream, logits, mask, nrouters, nexperts, weights);
-  return cudaGetLastError();
+  return launched(launch_pdl(router_weights_kernel, (nrouters + wpb - 1) / wpb, wpb * 32, 0, static_cast<cudaStream_t>(s),
+                             logits, mask, nrouters, nexperts, weights),
+                  "router_weights");
 }
 
 // y = sum_e w[e] * x_e with the reference's bf16 rounding after each multiply and add
+constexpr int kMaxRouterExperts = 8;
 struct RouterSources {  // expert tensors by value: nothing to stage on the device, so the launch is graph-capturable
   const __nv_bfloat16* p[kMaxRouterExperts];
 };
@@ -274,13 +284,15 @@ __global__ void router_merge_kernel(const __grid_constant__ RouterSources xs, co
                       pack_bf16x2(acc[6], acc[7]));
   }
 }
-cudaError_t launch_router_merge(const __nv_bfloat16* const* xs_host, const float* w, int nactive, long long n,
-                                __nv_bfloat16* y, cudaStream_t stream) {
-  if ((n & 7) || nactive < 1 || nactive > kMaxRouterExperts) return cudaErrorInvalidValue;
+extern "C" int ca_router_merge(const void* const* xs, const float* w, int32_t nactive, int64_t n, void* y, void* s) {
+  if (nactive < 1 || nactive > kMaxRouterExperts)
+    return fail(CA_ERR_INVALID, "router_merge: nactive must be 1..%d (got %d)", kMaxRouterExperts, nactive);
+  if (n & 7) return fail(CA_ERR_INVALID, "router_merge: n (%lld) must be a multiple of 8", (long long)n);
   RouterSources src{};
-  for (int k = 0; k < nactive; ++k) src.p[k] = xs_host[k];
-  CA_KERNEL_LAUNCH(router_merge_kernel, blocks_for(n / 8, 256), 256, 0, stream, src, w, nactive, n / 8, reinterpret_cast<uint4*>(y));
-  return cudaGetLastError();
+  for (int k = 0; k < nactive; ++k) src.p[k] = static_cast<const __nv_bfloat16*>(xs[k]);
+  return launched(launch_pdl(router_merge_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s), src, w,
+                             nactive, n / 8, static_cast<uint4*>(y)),
+                  "router_merge");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -312,12 +324,12 @@ __global__ void cfg_euler_kernel(const __nv_bfloat16* __restrict__ eu, const __n
     if (next_in) next_in[i] = __float2bfloat16_rn(xn / next_div);
   }
 }
-cudaError_t launch_cfg_euler(const __nv_bfloat16* eps_uncond, const __nv_bfloat16* eps_text, const float* latents_in,
-                             long long n, float guidance, const float* step_row, int round_latents_bf16,
-                             float* latents_out, __nv_bfloat16* model_in_next, cudaStream_t stream) {
-  CA_KERNEL_LAUNCH(cfg_euler_kernel, blocks_for(n, 256), 256, 0, stream, eps_uncond, eps_text, latents_in, n, guidance, step_row,
-                                                           round_latents_bf16, latents_out, model_in_next);
-  return cudaGetLastError();
+extern "C" int ca_cfg_euler(const void* eu, const void* et, const float* lat, int64_t n, float g, const float* step_row,
+                            int32_t round_latents_bf16, float* lat_out, void* next_in, void* s) {
+  return launched(launch_pdl(cfg_euler_kernel, blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const __nv_bfloat16*>(eu), static_cast<const __nv_bfloat16*>(et), lat, n, g,
+                             step_row, round_latents_bf16, lat_out, static_cast<__nv_bfloat16*>(next_in)),
+                  "cfg_euler");
 }
 // Euler, v-prediction, per-frame guidance (SVD loop, svd/pipelines/svd_controlnet_adapter_pipeline.py:781-787 with the
 // diffusers v0.27.2 EulerDiscreteScheduler.step): row = {t, sigma, sigma_next, sqrt(sigma_next^2+1)};
@@ -348,15 +360,17 @@ __global__ void cfg_euler_v_kernel(const __nv_bfloat16* __restrict__ eu, const _
     if (next_in) next_in[i] = __float2bfloat16_rn(xn / next_div);
   }
 }
-cudaError_t launch_cfg_euler_v(const __nv_bfloat16* eps_uncond, const __nv_bfloat16* eps_text, const float* latents_in,
-                               long long n, const float* guidance, int frames, long long frame_elems,
-                               const float* step_row, int round_latents_bf16, float* latents_out,
-                               __nv_bfloat16* model_in_next, cudaStream_t stream) {
-  if (frames < 1 || frame_elems < 1 || n % (static_cast<long long>(frames) * frame_elems) != 0) return cudaErrorInvalidValue;
-  CA_KERNEL_LAUNCH(cfg_euler_v_kernel, blocks_for(n, 256), 256, 0, stream, eps_uncond, eps_text, latents_in, n, guidance, frames,
-                                                             frame_elems, step_row, round_latents_bf16, latents_out,
-                                                             model_in_next);
-  return cudaGetLastError();
+extern "C" int ca_cfg_euler_v(const void* eu, const void* et, const float* lat, int64_t n, const float* guidance,
+                              int32_t frames, int64_t frame_elems, const float* step_row, int32_t round_latents_bf16,
+                              float* lat_out, void* next_in, void* s) {
+  if (frames < 1 || frame_elems < 1 || n % (static_cast<long long>(frames) * frame_elems) != 0)
+    return fail(CA_ERR_INVALID, "cfg_euler_v: n (%lld) must be a multiple of frames * frame_elems (%d * %lld)",
+                (long long)n, frames, (long long)frame_elems);
+  return launched(launch_pdl(cfg_euler_v_kernel, blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const __nv_bfloat16*>(eu), static_cast<const __nv_bfloat16*>(et), lat, n,
+                             guidance, frames, frame_elems, step_row, round_latents_bf16, lat_out,
+                             static_cast<__nv_bfloat16*>(next_in)),
+                  "cfg_euler_v");
 }
 // DDIM (eta 0): row = {t, alpha_prod_t, alpha_prod_prev, -}; epsilon- or v-prediction model output
 __global__ void cfg_ddim_kernel(const __nv_bfloat16* __restrict__ eu, const __nv_bfloat16* __restrict__ et,
@@ -401,12 +415,12 @@ __global__ void cfg_ddim_kernel(const __nv_bfloat16* __restrict__ eu, const __nv
     if (next_in) next_in[i] = __float2bfloat16_rn(xn);
   }
 }
-cudaError_t launch_cfg_ddim(const __nv_bfloat16* eps_uncond, const __nv_bfloat16* eps_text, const float* latents_in,
-                            long long n, float guidance, const float* step_row, int round_latents_bf16,
-                            int v_prediction, float* latents_out, __nv_bfloat16* model_in_next, cudaStream_t stream) {
-  CA_KERNEL_LAUNCH(cfg_ddim_kernel, blocks_for(n, 256), 256, 0, stream, eps_uncond, eps_text, latents_in, n, guidance, step_row,
-                                                          round_latents_bf16, v_prediction, latents_out, model_in_next);
-  return cudaGetLastError();
+extern "C" int ca_cfg_ddim(const void* eu, const void* et, const float* lat, int64_t n, float g, const float* step_row,
+                           int32_t round_latents_bf16, int32_t v_prediction, float* lat_out, void* next_in, void* s) {
+  return launched(launch_pdl(cfg_ddim_kernel, blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const __nv_bfloat16*>(eu), static_cast<const __nv_bfloat16*>(et), lat, n, g,
+                             step_row, round_latents_bf16, v_prediction, lat_out, static_cast<__nv_bfloat16*>(next_in)),
+                  "cfg_ddim");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -487,13 +501,14 @@ __global__ void i2vgen_latent_encoder_kernel(const __nv_bfloat16* __restrict__ x
     }
   }
 }
-cudaError_t launch_i2vgen_latent_encoder(const __nv_bfloat16* x, int clips, int frames, long long hw, int c_stride,
-                                         const float* params, __nv_bfloat16* y, cudaStream_t stream) {
-  if (frames > 32 || frames < 1) return cudaErrorInvalidValue;
+extern "C" int ca_i2vgen_latent_encoder(const void* x, int32_t clips, int32_t frames, int64_t hw, int32_t c_stride,
+                                        const float* params, void* y, void* s) {
+  if (frames < 1 || frames > 32) return fail(CA_ERR_INVALID, "i2vgen_latent_encoder: frames must be 1..32 (got %d)", frames);
   const long long total = static_cast<long long>(clips) * hw;
-  CA_KERNEL_LAUNCH(i2vgen_latent_encoder_kernel, static_cast<unsigned>((total + 63) / 64), 64, 0, stream, x, frames, hw, c_stride,
-                                                                                          params, total, y);
-  return cudaGetLastError();
+  return launched(launch_pdl(i2vgen_latent_encoder_kernel, static_cast<unsigned>((total + 63) / 64), 64, 0,
+                             static_cast<cudaStream_t>(s), static_cast<const __nv_bfloat16*>(x), frames, hw, c_stride,
+                             params, total, static_cast<__nv_bfloat16*>(y)),
+                  "i2vgen_latent_encoder");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -504,6 +519,11 @@ cudaError_t launch_i2vgen_latent_encoder(const __nv_bfloat16* x, int clips, int 
 // planes of the logical NCHW result directly (the layout conversion is fused).  fp32 accumulation, one rounding to bf16.
 // The 27 + 3 parameters travel in the kernel parameter space.
 // ---------------------------------------------------------------------------------------------
+constexpr int kFrameConvMaxC = 4;
+struct FrameConvSmallParams {
+  float w[kFrameConvMaxC][kFrameConvMaxC][3];  // [out channel][in channel][frame tap]
+  float b[kFrameConvMaxC];
+};
 __global__ void __launch_bounds__(256)
 frame_conv_small_kernel(const __nv_bfloat16* __restrict__ x, int frames, long long hw, int c_stride, int cin, int cout,
                         FrameConvSmallParams prm, __nv_bfloat16* __restrict__ y) {
@@ -546,12 +566,17 @@ frame_conv_small_kernel(const __nv_bfloat16* __restrict__ x, int frames, long lo
     }
   }
 }
-cudaError_t launch_frame_conv_small(const __nv_bfloat16* x, int clips, int frames, long long hw, int c_stride, int cin,
-                                    int cout, const float* w_host, const float* bias_host, __nv_bfloat16* y,
-                                    cudaStream_t stream) {
-  if (clips < 1 || frames < 1 || hw < 1 || cin < 1 || cout < 1 || cin > kFrameConvMaxC || cout > kFrameConvMaxC ||
-      c_stride < 4 || (c_stride & 3) != 0 || static_cast<long long>(clips) * frames > 65535)
-    return cudaErrorInvalidValue;
+extern "C" int ca_frame_conv_small(const void* x, int32_t clips, int32_t frames, int64_t hw, int32_t c_stride,
+                                   int32_t cin, int32_t cout, const float* w_host, const float* bias_host, void* y,
+                                   void* s) {
+  if (w_host == nullptr) return fail(CA_ERR_INVALID, "frame_conv_small: null weight pointer");
+  if (cin < 1 || cout < 1 || cin > kFrameConvMaxC || cout > kFrameConvMaxC)
+    return fail(CA_ERR_INVALID, "frame_conv_small: cin, cout (%d, %d) must be 1..%d", cin, cout, kFrameConvMaxC);
+  if (c_stride < 4 || (c_stride & 3) != 0)
+    return fail(CA_ERR_INVALID, "frame_conv_small: c_stride (%d) must be a positive multiple of 4", c_stride);
+  if (clips < 1 || frames < 1 || hw < 1 || static_cast<long long>(clips) * frames > 65535)
+    return fail(CA_ERR_INVALID, "frame_conv_small: clips, frames, hw (%d, %d, %lld) must be positive with clips * frames "
+                "<= 65535", clips, frames, (long long)hw);
   FrameConvSmallParams prm = {};
   for (int co = 0; co < cout; ++co) {
     prm.b[co] = bias_host != nullptr ? bias_host[co] : 0.f;
@@ -559,8 +584,10 @@ cudaError_t launch_frame_conv_small(const __nv_bfloat16* x, int clips, int frame
       for (int dt = 0; dt < 3; ++dt) prm.w[co][ci][dt] = w_host[(co * cin + ci) * 3 + dt];
   }
   const dim3 grid(static_cast<unsigned>((hw + 511) / 512), static_cast<unsigned>(clips * frames));
-  CA_KERNEL_LAUNCH(frame_conv_small_kernel, grid, 256, 0, stream, x, frames, hw, c_stride, cin, cout, prm, y);
-  return cudaGetLastError();
+  return launched(launch_pdl(frame_conv_small_kernel, grid, 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const __nv_bfloat16*>(x), frames, hw, c_stride, cin, cout, prm,
+                             static_cast<__nv_bfloat16*>(y)),
+                  "frame_conv_small");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -611,138 +638,12 @@ softmax_rows_kernel(const float* __restrict__ x, long long cols, __nv_bfloat16* 
                         pack_bf16x2(__expf(v.z - m) * inv, __expf(v.w - m) * inv));
   }
 }
-cudaError_t launch_softmax_rows(const float* x, long long rows, long long cols, __nv_bfloat16* y, cudaStream_t stream) {
-  if (rows < 1 || rows > 0x7fffffffLL || cols < 4 || (cols & 3) != 0) return cudaErrorInvalidValue;
-  CA_KERNEL_LAUNCH(softmax_rows_kernel, static_cast<unsigned>(rows), 256, 0, stream, x, cols, y);
-  return cudaGetLastError();
-}
-
-// ---------------------------------------------------------------------------------------------
-// Temporal self-attention: sequence = the F frames of one pixel, head dim 64.  HBM-bound (every Q/K/V element is read
-// once), so plain FMA.  One warp per (clip, pixel, head).
-//   frames <= 16: lane = (query frame i = lane >> 1, half = lane & 1 of the head dim): each lane holds q[i][32 dims],
-//                 walks the F keys (K rows are shared by all lanes -> L1 broadcast), one shuffle per score to join
-//                 the two halves, softmax over <= 16 scores in registers, then accumulates its 32 output dims.
-//   frames <= 32: lane = query frame, full 64 dims per lane (no shuffles).
-// Layout [clip][frame][pixel][row stride]; output dense [.., heads*64].
-// ---------------------------------------------------------------------------------------------
-template <int HALVES>  // 2: two lanes per frame (frames <= 16); 1: one lane per frame (frames <= 32)
-__global__ void __launch_bounds__(128)
-temporal_attention_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
-                          const __nv_bfloat16* __restrict__ v, int frames, long long hw, int heads, float scale,
-                          long long in_stride, long long total_warps, __nv_bfloat16* __restrict__ out) {
-  CA_PDL_TRIGGER();
-  CA_PDL_WAIT();
-  constexpr int D = 64 / HALVES;        // head-dim elements owned by a lane
-  constexpr int MAXF = 32 / HALVES;     // max frames
-  const long long wid = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
-  if (wid >= total_warps) return;
-  const int lane = threadIdx.x & 31;
-  const int head = static_cast<int>(wid % heads);
-  long long t = wid / heads;
-  const long long pix = t % hw;
-  const long long clip = t / hw;
-  const long long cstride = static_cast<long long>(heads) * 64;
-  const long long fstride = hw * in_stride;   // input frame stride (rows may be views of a fused QKV buffer)
-  const long long ofstride = hw * cstride;    // output is dense
-  const int fi = lane / HALVES;               // query frame of this lane
-  const int half = lane % HALVES;
-  const bool active = fi < frames;
-  const long long base = (clip * frames * hw + pix) * in_stride + head * 64 + half * D;
-  const long long obase = (clip * frames * hw + pix) * cstride + head * 64 + half * D;
-  float qf[D];
-  {
-    const int fq = active ? fi : 0;
-    const uint4* qp = reinterpret_cast<const uint4*>(q + base + fq * fstride);
-#pragma unroll
-    for (int u = 0; u < D / 8; ++u) {
-      const uint4 w = __ldg(qp + u);
-      const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&w);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 f = __bfloat1622float2(h2[e]);
-        qf[u * 8 + 2 * e] = f.x * scale;
-        qf[u * 8 + 2 * e + 1] = f.y * scale;
-      }
-    }
-  }
-  float s[MAXF];
-  float mx = -INFINITY;
-#pragma unroll
-  for (int j = 0; j < MAXF; ++j) {
-    s[j] = -INFINITY;
-    if (j < frames) {
-      const uint4* kp = reinterpret_cast<const uint4*>(k + base + j * fstride);
-      float d = 0.f;
-#pragma unroll
-      for (int u = 0; u < D / 8; ++u) {
-        const uint4 w = __ldg(kp + u);
-        const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&w);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 f = __bfloat1622float2(h2[e]);
-          d = fmaf(qf[u * 8 + 2 * e], f.x, d);
-          d = fmaf(qf[u * 8 + 2 * e + 1], f.y, d);
-        }
-      }
-      if (HALVES == 2) d += __shfl_xor_sync(0xffffffffu, d, 1);
-      s[j] = d;
-      mx = fmaxf(mx, d);
-    }
-  }
-  float l = 0.f;
-#pragma unroll
-  for (int j = 0; j < MAXF; ++j) {
-    if (j < frames) {
-      const float pe = __expf(s[j] - mx);
-      l += pe;
-      s[j] = round_bf16(pe);  // P is bf16 in the fused SDPA kernels of the reference path
-    }
-  }
-  float o[D];
-#pragma unroll
-  for (int e = 0; e < D; ++e) o[e] = 0.f;
-#pragma unroll
-  for (int j = 0; j < MAXF; ++j) {
-    if (j < frames) {
-      const uint4* vp = reinterpret_cast<const uint4*>(v + base + j * fstride);
-      const float pj = s[j];
-#pragma unroll
-      for (int u = 0; u < D / 8; ++u) {
-        const uint4 w = __ldg(vp + u);
-        const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&w);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 f = __bfloat1622float2(h2[e]);
-          o[u * 8 + 2 * e] = fmaf(pj, f.x, o[u * 8 + 2 * e]);
-          o[u * 8 + 2 * e + 1] = fmaf(pj, f.y, o[u * 8 + 2 * e + 1]);
-        }
-      }
-    }
-  }
-  if (active) {
-    const float inv = 1.0f / l;
-    uint4* op = reinterpret_cast<uint4*>(out + obase + fi * ofstride);
-#pragma unroll
-    for (int u = 0; u < D / 8; ++u)
-      op[u] = make_uint4(pack_bf16x2(o[u * 8] * inv, o[u * 8 + 1] * inv), pack_bf16x2(o[u * 8 + 2] * inv, o[u * 8 + 3] * inv),
-                         pack_bf16x2(o[u * 8 + 4] * inv, o[u * 8 + 5] * inv), pack_bf16x2(o[u * 8 + 6] * inv, o[u * 8 + 7] * inv));
-  }
-}
-cudaError_t launch_temporal_attention(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, int clips,
-                                      int frames, long long hw, int heads, float scale, long long in_row_stride,
-                                      __nv_bfloat16* out, cudaStream_t stream) {
-  if (frames > 32 || frames < 1 || (in_row_stride & 7) != 0) return cudaErrorInvalidValue;
-  const long long total_warps = static_cast<long long>(clips) * hw * heads;
-  const int threads = 128;
-  const long long blocks = (total_warps * 32 + threads - 1) / threads;
-  if (frames <= 16)
-    CA_KERNEL_LAUNCH(temporal_attention_kernel<2>, static_cast<unsigned>(blocks), threads, 0, stream, q, k, v, frames, hw, heads, scale,
-                                                                                       in_row_stride, total_warps, out);
-  else
-    CA_KERNEL_LAUNCH(temporal_attention_kernel<1>, static_cast<unsigned>(blocks), threads, 0, stream, q, k, v, frames, hw, heads, scale,
-                                                                                       in_row_stride, total_warps, out);
-  return cudaGetLastError();
+extern "C" int ca_softmax_rows(const float* x, int64_t rows, int64_t cols, void* y, void* s) {
+  if (rows < 1 || rows > 0x7fffffffLL) return fail(CA_ERR_INVALID, "softmax_rows: rows (%lld) must be 1..2^31-1", (long long)rows);
+  if (cols < 4 || (cols & 3) != 0) return fail(CA_ERR_INVALID, "softmax_rows: cols (%lld) must be a positive multiple of 4", (long long)cols);
+  return launched(launch_pdl(softmax_rows_kernel, static_cast<unsigned>(rows), 256, 0, static_cast<cudaStream_t>(s), x,
+                             cols, static_cast<__nv_bfloat16*>(y)),
+                  "softmax_rows");
 }
 
 }  // namespace ca

@@ -13,7 +13,7 @@
 //                             it runs ahead into the next tile's ring slots while the current tile is written out
 //   warpgroup 0, warps 1-3  : storers (bf16 outputs).  Per tile: wait on `staged`, then read the staged tile, add
 //                             row vector / residual / AlphaBlender with their bf16 roundings and write the output with
-//                             16-byte loads and stores (element-wise when capi.cu finds a pointer or stride that is
+//                             16-byte loads and stores (element-wise when ca_gemm finds a pointer or stride that is
 //                             not 16-byte aligned), skipping rows outside the output box; then arrive on `drained`
 //   warpgroups 1, 2         : consumers.  Warpgroup g issues m64nBNk16 wgmma for rows [64g, 64g + 64) of the tile with
 //                             both operands read from the 128B-swizzled ring, accumulates in registers, and releases
@@ -473,8 +473,7 @@ static cudaError_t launch_epi(const CUtensorMap& a0, const CUtensorMap& a1, cons
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  CA_KERNEL_LAUNCH(kern, grid, kGemmThreads, Cfg::kSmemBytes, stream, a0, a1, w, p);
-  return cudaGetLastError();
+  return launch_pdl(kern, grid, kGemmThreads, Cfg::kSmemBytes, stream, a0, a1, w, p);
 }
 
 // one translation unit per BN (gemm_conv_bn*.cu) instantiates its kernels through this

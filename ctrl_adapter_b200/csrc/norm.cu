@@ -90,12 +90,23 @@ gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, const __nv_bfloat1
     atomicAdd(&sums[static_cast<long long>(n) * groups * 2 + i], static_cast<double>((&s_acc[0][0])[i]));
 }
 
-cudaError_t launch_gn_stats(const __nv_bfloat16* x0, int c0, const __nv_bfloat16* x1, int c1, int n, long long rows,
-                            int groups, double* sums, cudaStream_t stream) {
+// the GroupNorm channel layout both passes support: <= 64 groups of whole 8-channel vectors, <= 512 vectors per pixel
+static int check_gn_channels(const char* what, int c0, int c1, int groups) {
   const int C = c0 + c1;
-  if (groups > 64 || C % groups != 0 || (C & 7) != 0 || (c0 & 7) != 0 || (C >> 3) > 512) return cudaErrorInvalidValue;
+  if (groups < 1 || groups > 64) return fail(CA_ERR_INVALID, "%s: groups must be 1..64 (got %d)", what, groups);
+  if (C % groups != 0) return fail(CA_ERR_INVALID, "%s: c0 + c1 (%d) must be a multiple of groups (%d)", what, C, groups);
+  if ((c0 & 7) != 0 || (c1 & 7) != 0 || C < 8 || C > 4096)
+    return fail(CA_ERR_INVALID, "%s: c0, c1 (%d, %d) must be multiples of 8 with 8 <= c0 + c1 <= 4096", what, c0, c1);
+  return CA_OK;
+}
+
+extern "C" int ca_groupnorm_stats(const void* x0, int32_t c0, const void* x1, int32_t c1, int32_t n, int64_t rows,
+                                  int32_t groups, double* sums, void* s) {
+  if (int rc = check_gn_channels("groupnorm_stats", c0, c1, groups)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(s);
   cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * n * groups * 2, stream);
-  if (e != cudaSuccess) return e;
+  if (e != cudaSuccess) return launched(e, "groupnorm_stats");
+  const int C = c0 + c1;
   const int threads = 512;
   // >= ~4 resident blocks per SM overall, while keeping the per-thread fp32 partial sums short (<= ~64 rows)
   const int rows_per_iter = threads / (C >> 3);
@@ -105,8 +116,9 @@ cudaError_t launch_gn_stats(const __nv_bfloat16* x0, int c0, const __nv_bfloat16
   if (rpb < min_rpb) rpb = min_rpb;
   if (rpb > max_rpb) rpb = max_rpb;
   const int slabs = static_cast<int>((rows + rpb - 1) / rpb);
-  CA_KERNEL_LAUNCH(gn_stats_kernel, dim3(slabs, n), threads, 0, stream, x0, c0, x1, c1, rows, groups, static_cast<int>(rpb), sums);
-  return cudaGetLastError();
+  e = launch_pdl(gn_stats_kernel, dim3(slabs, n), threads, 0, stream, static_cast<const __nv_bfloat16*>(x0), c0,
+                 static_cast<const __nv_bfloat16*>(x1), c1, rows, groups, static_cast<int>(rpb), sums);
+  return launched(e, "groupnorm_stats");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -214,13 +226,13 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, const __nv_bfloat1
   for (; pix < p_end; pix += rows_per_iter) emit(ld_nc(src + static_cast<long long>(pix) * cs), pix);
 }
 
-cudaError_t launch_gn_apply(const __nv_bfloat16* x0, int c0, const __nv_bfloat16* x1, int c1, int n, int h, int w,
-                            int imgs_per_sample, int groups, float eps, const double* sums, const float* gamma,
-                            const float* beta, int silu, int up2x, __nv_bfloat16* y, cudaStream_t stream) {
-  const int C = c0 + c1;
-  if (groups > 64 || C % groups != 0 || (C & 7) != 0 || (c0 & 7) != 0 || C > 4096) return cudaErrorInvalidValue;
+extern "C" int ca_groupnorm_apply(const void* x0, int32_t c0, const void* x1, int32_t c1, int32_t n, int32_t h,
+                                  int32_t w, int32_t imgs_per_sample, int32_t groups, float eps, const double* sums,
+                                  const float* gamma, const float* beta, int32_t silu, int32_t up2x, void* y, void* s) {
+  if (int rc = check_gn_channels("groupnorm_apply", c0, c1, groups)) return rc;
   const long long hw = static_cast<long long>(h) * w;
-  if (hw > 0x3fffffffLL) return cudaErrorInvalidValue;
+  if (hw > 0x3fffffffLL) return fail(CA_ERR_INVALID, "groupnorm_apply: h * w (%lld) must be < 2^30", hw);
+  const int C = c0 + c1;
   const int nvec = C >> 3;
   const int rows_per_iter = 512 / nvec;  // >= 1 because C <= 4096
   const int threads = rows_per_iter * nvec;
@@ -230,20 +242,13 @@ cudaError_t launch_gn_apply(const __nv_bfloat16* x0, int c0, const __nv_bfloat16
   long long ppb = ((hw + want_blocks - 1) / want_blocks + step - 1) / step * step;
   if (ppb < 2 * step) ppb = 2 * step;
   const int slabs = static_cast<int>((hw + ppb - 1) / ppb);
-  const dim3 grid(slabs, n);
-#define CA_GN(S, U)                                                                                               \
-  do {                                                                                                            \
-    auto kern = gn_apply_kernel<S, U>;                                                                            \
-    CA_KERNEL_LAUNCH(kern, grid, threads, 0, stream, x0, c0, x1, c1, h, w, imgs_per_sample, groups, eps, sums, gamma, \
-                     beta, static_cast<int>(ppb), y);                                                             \
-  } while (0)
-  if (silu) {
-    if (up2x) CA_GN(true, true); else CA_GN(true, false);
-  } else {
-    if (up2x) CA_GN(false, true); else CA_GN(false, false);
-  }
-#undef CA_GN
-  return cudaGetLastError();
+  auto kern = silu ? (up2x ? gn_apply_kernel<true, true> : gn_apply_kernel<true, false>)
+                   : (up2x ? gn_apply_kernel<false, true> : gn_apply_kernel<false, false>);
+  const cudaError_t e = launch_pdl(kern, dim3(slabs, n), threads, 0, static_cast<cudaStream_t>(s),
+                                   static_cast<const __nv_bfloat16*>(x0), c0, static_cast<const __nv_bfloat16*>(x1), c1,
+                                   h, w, imgs_per_sample, groups, eps, sums, gamma, beta, static_cast<int>(ppb),
+                                   static_cast<__nv_bfloat16*>(y));
+  return launched(e, "groupnorm_apply");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -259,7 +264,6 @@ cudaError_t launch_gn_apply(const __nv_bfloat16* x0, int c0, const __nv_bfloat16
 //  * Statistics in ONE pass over d = x - K with K = the row's first element: mean = K + sum(d)/C,
 //    var = (sum(d^2) - sum(d)^2 / C) / C.  K is an element of the row, so (K - mean)^2 <= (C - 1) var and the
 //    cancellation costs at most ~C ulp of fp32 in var (1.5e-4 relative at C = 1280), far below the bf16 output grid.
-//  * Arithmetic on packed fp32x2 (FADD2 / FFMA2 / FMUL2).
 // RV: fused pre-add of a broadcast row vector (frame position embedding / single-token cross-attention output),
 // rounded to bf16 like the eager add it replaces, written back into the stage; optionally also written out (y_sum).
 // ---------------------------------------------------------------------------------------------
@@ -306,23 +310,23 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
     fence_proxy_async_smem();
   }
   __syncwarp();
-  auto load_gb = [&](int v, uint64_t (&g)[4], uint64_t (&b)[4]) {
+  auto load_gb = [&](int v, float (&g)[8], float (&b)[8]) {
     const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + v * 8));
     const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + v * 8) + 1);
     const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + v * 8));
     const float4 b1 = __ldg(reinterpret_cast<const float4*>(beta + v * 8) + 1);
-    g[0] = pack_f32x2(g0.x, g0.y); g[1] = pack_f32x2(g0.z, g0.w); g[2] = pack_f32x2(g1.x, g1.y); g[3] = pack_f32x2(g1.z, g1.w);
-    b[0] = pack_f32x2(b0.x, b0.y); b[1] = pack_f32x2(b0.z, b0.w); b[2] = pack_f32x2(b1.x, b1.y); b[3] = pack_f32x2(b1.z, b1.w);
+    g[0] = g0.x; g[1] = g0.y; g[2] = g0.z; g[3] = g0.w; g[4] = g1.x; g[5] = g1.y; g[6] = g1.z; g[7] = g1.w;
+    b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
   };
   // vector k of this lane is column block v = ll + L k; only the last k can fall off the end of the row
   auto has = [&](int k) { return k < NV - 1 || ll + L * k < nvec; };
   // parameters, not produced by the previous kernel: loaded ahead of the programmatic-launch wait
-  [[maybe_unused]] uint64_t gg[kHold ? NV : 1][4], bb[kHold ? NV : 1][4];
+  [[maybe_unused]] float gg[kHold ? NV : 1][8], bb[kHold ? NV : 1][8];
   if constexpr (kHold) {
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) gg[k][e] = bb[k][e] = 0;
+      for (int e = 0; e < 8; ++e) gg[k][e] = bb[k][e] = 0.f;
       if (has(k)) load_gb(ll + L * k, gg[k], bb[k]);
     }
   }
@@ -345,7 +349,6 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
     for (int s = 0; s < kLnStages; ++s)
       if (step0 + s * step_stride < steps) fill(s, step0 + s * step_stride);
   }
-  auto widen = [](uint32_t w) { return pack_f32x2(bf16lo_to_float(w), bf16hi_to_float(w)); };
   const float inv_c = 1.f / static_cast<float>(c);
   uint32_t stage = 0, phase = 0;
   for (int step = step0; step < steps; step += step_stride) {
@@ -360,9 +363,8 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(kw) : "r"(srow - ll * 16));
     if constexpr (RV) kw = add_bf16x2(kw, __ldg(reinterpret_cast<const uint32_t*>(av)));
     const float shift = bf16lo_to_float(kw);
-    const uint64_t nshift2 = pack_f32x2(-shift, -shift);
-    // pass 1: sum and sum of squares of d = x - K (and the fused row-vector add)
-    uint64_t s2 = pack_f32x2(0.f, 0.f), ss2 = pack_f32x2(0.f, 0.f);
+    // pass 1: sum and sum of squares of d = x - K (and the fused row-vector add), even / odd columns apart
+    float s_lo = 0.f, s_hi = 0.f, ss_lo = 0.f, ss_hi = 0.f;
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
       if (has(k)) {
@@ -380,15 +382,15 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
         const uint32_t wds[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const uint64_t d = add_f32x2(widen(wds[e]), nshift2);
-          s2 = add_f32x2(s2, d);
-          ss2 = fma_f32x2(d, d, ss2);
+          const float d_lo = __fadd_rn(bf16lo_to_float(wds[e]), -shift);
+          const float d_hi = __fadd_rn(bf16hi_to_float(wds[e]), -shift);
+          s_lo = __fadd_rn(s_lo, d_lo);
+          s_hi = __fadd_rn(s_hi, d_hi);
+          ss_lo = __fmaf_rn(d_lo, d_lo, ss_lo);
+          ss_hi = __fmaf_rn(d_hi, d_hi, ss_hi);
         }
       }
     }
-    float s_lo, s_hi, ss_lo, ss_hi;
-    unpack_f32x2(s2, s_lo, s_hi);
-    unpack_f32x2(ss2, ss_lo, ss_hi);
     float sd = s_lo + s_hi, sq = ss_lo + ss_hi;
 #pragma unroll
     for (int o = L / 2; o > 0; o >>= 1) {
@@ -399,8 +401,6 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
     const float var = fmaxf((sq - sd * mean_d) * inv_c, 0.f);
     const float mean = shift + mean_d;
     const float rstd = rsqrtf(var + eps);
-    const uint64_t nmean2 = pack_f32x2(-mean, -mean);
-    const uint64_t rstd2 = pack_f32x2(rstd, rstd);
     // pass 2: normalise, scale, shift, store
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
@@ -408,17 +408,20 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
         const int v = ll + L * k;
         const uint4 q = lds128(srow + 16 * L * k);
         const uint32_t wds[4] = {q.x, q.y, q.z, q.w};
-        [[maybe_unused]] uint64_t g1[4], b1[4];
-        if constexpr (!kHold) load_gb(v, g1, b1);
+        float ge[8], be[8];
+        if constexpr (kHold) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) { ge[i] = gg[k][i]; be[i] = bb[k][i]; }
+        } else {
+          load_gb(v, ge, be);
+        }
         uint32_t o[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const uint64_t ge = kHold ? gg[kHold ? k : 0][e] : g1[e];
-          const uint64_t be = kHold ? bb[kHold ? k : 0][e] : b1[e];
           // ((x - mean) * rstd) * gamma + beta, the association of the eager kernel
-          const uint64_t r = fma_f32x2(mul_f32x2(add_f32x2(widen(wds[e]), nmean2), rstd2), ge, be);
-          float r0, r1;
-          unpack_f32x2(r, r0, r1);
+          const float r0 = __fmaf_rn(__fmul_rn(__fadd_rn(bf16lo_to_float(wds[e]), -mean), rstd), ge[2 * e], be[2 * e]);
+          const float r1 =
+              __fmaf_rn(__fmul_rn(__fadd_rn(bf16hi_to_float(wds[e]), -mean), rstd), ge[2 * e + 1], be[2 * e + 1]);
           o[e] = pack_bf16x2(r0, r1);
         }
         if (row_ok) *reinterpret_cast<uint4*>(y + static_cast<long long>(row) * c + v * 8) = make_uint4(o[0], o[1], o[2], o[3]);
@@ -439,11 +442,10 @@ layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long rows, int c, flo
   }
 }
 
-namespace {
 template <int NV, int L>
-cudaError_t launch_layernorm_t(const __nv_bfloat16* x, long long rows, int c, float eps, const float* gamma,
-                               const float* beta, const __nv_bfloat16* add_rowvec, long long rpv, __nv_bfloat16* y_sum,
-                               __nv_bfloat16* y, int sms, cudaStream_t stream) {
+static cudaError_t launch_layernorm(const __nv_bfloat16* x, long long rows, int c, float eps, const float* gamma,
+                                   const float* beta, const __nv_bfloat16* add_rowvec, long long rpv,
+                                   __nv_bfloat16* y_sum, __nv_bfloat16* y, cudaStream_t stream) {
   constexpr int G = 32 / L;
   static bool optin = false;  // the ring can exceed the 48 KB default: opt both variants in once
   if (!optin) {
@@ -460,29 +462,27 @@ cudaError_t launch_layernorm_t(const __nv_bfloat16* x, long long rows, int c, fl
   int per_sm = ln_blocks_per_sm(NV);
   const int by_smem = static_cast<int>((228u * 1024u) / (smem + 1024u));
   if (by_smem < per_sm) per_sm = by_smem;
-  const long long resident = static_cast<long long>(sms) * per_sm;
+  const long long resident = static_cast<long long>(num_sms()) * per_sm;
   const long long steps = (rows + G - 1) / G;
   const long long need = (steps + kLnWarps - 1) / kLnWarps;
   const unsigned blocks = static_cast<unsigned>(need < resident ? need : resident);
   auto kern = (add_rowvec != nullptr) ? layernorm_kernel<NV, L, true> : layernorm_kernel<NV, L, false>;
-  CA_KERNEL_LAUNCH(kern, blocks, kLnWarps * 32, smem, stream, x, rows, c, eps, gamma, beta, add_rowvec, rpv, y_sum, y);
-  return cudaGetLastError();
+  return launch_pdl(kern, blocks, kLnWarps * 32, smem, stream, x, rows, c, eps, gamma, beta, add_rowvec, rpv, y_sum, y);
 }
-}  // namespace
 
-cudaError_t launch_layernorm(const __nv_bfloat16* x, long long rows, int c, float eps, const float* gamma,
-                             const float* beta, const __nv_bfloat16* add_rowvec, long long rows_per_vec,
-                             __nv_bfloat16* y_sum, __nv_bfloat16* y, cudaStream_t stream) {
-  if ((c & 7) != 0 || c < 8 || c > kLnMaxC) return cudaErrorInvalidValue;
-  if ((reinterpret_cast<uintptr_t>(x) & 15) != 0) return cudaErrorMisalignedAddress;  // bulk copies of whole rows
-  if (rows <= 0) return cudaSuccess;
-  if (rows >= (1LL << 31) - 64) return cudaErrorInvalidValue;
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) sms = 148;
-  }
+extern "C" int ca_layernorm(const void* x_, int64_t rows, int32_t c, float eps, const float* gamma, const float* beta,
+                            const void* add_rowvec_, int64_t rows_per_vec, void* y_sum_, void* y_, void* s) {
+  if ((c & 7) != 0 || c < 8 || c > kLnMaxC)
+    return fail(CA_ERR_INVALID, "layernorm: c (%d) must be a multiple of 8 in 8..%d", c, kLnMaxC);
+  // whole rows travel as 1-D bulk copies
+  if ((reinterpret_cast<uintptr_t>(x_) & 15) != 0) return fail(CA_ERR_INVALID, "layernorm: x must be 16-byte aligned");
+  if (rows <= 0) return CA_OK;
+  if (rows >= (1LL << 31) - 64) return fail(CA_ERR_INVALID, "layernorm: rows (%lld) must be < 2^31 - 64", (long long)rows);
+  const auto* x = static_cast<const __nv_bfloat16*>(x_);
+  const auto* add_rowvec = static_cast<const __nv_bfloat16*>(add_rowvec_);
+  auto* y_sum = static_cast<__nv_bfloat16*>(y_sum_);
+  auto* y = static_cast<__nv_bfloat16*>(y_);
+  cudaStream_t stream = static_cast<cudaStream_t>(s);
   const long long rpv = rows_per_vec > 0 ? rows_per_vec : 1;
   const int nvec = c >> 3;
   // the narrowest lane group that still keeps gamma / beta in registers
@@ -491,7 +491,7 @@ cudaError_t launch_layernorm(const __nv_bfloat16* x, long long rows, int c, floa
   else if ((nvec + 15) / 16 <= kLnHoldMaxNV) lanes = 16;
   const int nv = (nvec + lanes - 1) / lanes;
 #define CA_LN(NV, L) \
-  return launch_layernorm_t<NV, L>(x, rows, c, eps, gamma, beta, add_rowvec, rpv, y_sum, y, sms, stream)
+  return launched(launch_layernorm<NV, L>(x, rows, c, eps, gamma, beta, add_rowvec, rpv, y_sum, y, stream), "layernorm")
   if (lanes == 8) {
     switch (nv) {
       case 1: CA_LN(1, 8);

@@ -21,6 +21,14 @@ static constexpr int kTaThreads = 128;
 static constexpr uint32_t kTaTile = 128 * 64 * 2;  // one [128 rows x 64 dims] bf16 tile = 16 KB
 static constexpr uint32_t kTaSmem = 3 * kTaTile + 1024 /*align slack*/ + 64 /*barrier*/;
 
+struct TemporalAttnParams {
+  int clips, frames, heads;
+  long long hw;
+  float scale_log2;            // softmax scale * log2(e)
+  __nv_bfloat16* out;          // rows ((clip * frames + f) * hw + pixel), heads * 64 used columns
+  long long out_row_stride;    // elements
+};
+
 template <int SEQ>
 __global__ void __launch_bounds__(kTaThreads)
 temporal_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
@@ -143,7 +151,7 @@ temporal_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const _
 
 template <int SEQ>
 static cudaError_t launch_seq(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v,
-                              const TemporalAttnParams& p, cudaStream_t stream) {
+                              const TemporalAttnParams& p, long long ctas, cudaStream_t stream) {
   static bool attr_set = false;
   auto kern = temporal_attention_tc_kernel<SEQ>;
   if (!attr_set) {
@@ -151,17 +159,36 @@ static cudaError_t launch_seq(const CUtensorMap& q, const CUtensorMap& k, const 
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const long long groups = (p.hw + 128 / SEQ - 1) / (128 / SEQ);
-  const long long total = static_cast<long long>(p.clips) * groups * p.heads;
-  if (total <= 0 || total > 0x7fffffffLL) return cudaErrorInvalidValue;
-  CA_KERNEL_LAUNCH(kern, static_cast<unsigned>(total), kTaThreads, kTaSmem, stream, q, k, v, p);
-  return cudaGetLastError();
+  return launch_pdl(kern, static_cast<unsigned>(ctas), kTaThreads, kTaSmem, stream, q, k, v, p);
 }
 
-cudaError_t launch_temporal_attention_tc(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v,
-                                         const TemporalAttnParams& p, cudaStream_t stream) {
-  if (p.frames < 1 || p.frames > 32) return cudaErrorInvalidValue;
-  return p.frames <= 16 ? launch_seq<16>(q, k, v, p, stream) : launch_seq<32>(q, k, v, p, stream);
+extern "C" int ca_temporal_attention(const void* q, const void* k, const void* v, int32_t clips, int32_t frames,
+                                     int64_t hw, int32_t heads, float scale, int64_t in_row_stride, void* out, void* s) {
+  if (frames < 1 || frames > 32) return fail(CA_ERR_INVALID, "temporal_attention: frames must be 1..32 (got %d)", frames);
+  if (clips < 1 || hw < 1 || heads < 1) return fail(CA_ERR_INVALID, "temporal_attention: empty problem (clips, hw, heads)");
+  if ((in_row_stride & 7) != 0) return fail(CA_ERR_INVALID, "temporal_attention: in_row_stride must be a multiple of 8");
+  // one CTA per (clip, group of 128 / SEQ pixels, head)
+  const int seq = frames <= 16 ? 16 : 32;
+  const long long ctas = static_cast<long long>(clips) * ((hw + 128 / seq - 1) / (128 / seq)) * heads;
+  if (ctas > 0x7fffffffLL) return fail(CA_ERR_INVALID, "temporal_attention: clips * hw * heads too large");
+  // global dims ordered (channel, frame, pixel, clip): a box then holds whole frame sequences of consecutive pixels
+  const cuuint64_t dims[4] = {(cuuint64_t)heads * 64, (cuuint64_t)frames, (cuuint64_t)hw, (cuuint64_t)clips};
+  const cuuint64_t st[3] = {(cuuint64_t)hw * in_row_stride * 2, (cuuint64_t)in_row_stride * 2,
+                            (cuuint64_t)frames * hw * in_row_stride * 2};
+  const cuuint32_t box[4] = {64, (cuuint32_t)seq, (cuuint32_t)(128 / seq), 1};
+  CUtensorMap tq, tk, tv;
+  int rc = make_tmap(&tq, q, 4, dims, st, box);
+  if (rc) return rc;
+  if ((rc = make_tmap(&tk, k, 4, dims, st, box))) return rc;
+  if ((rc = make_tmap(&tv, v, 4, dims, st, box))) return rc;
+  TemporalAttnParams p;
+  p.clips = clips; p.frames = frames; p.heads = heads; p.hw = hw;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.out_row_stride = static_cast<long long>(heads) * 64;
+  cudaStream_t stream = static_cast<cudaStream_t>(s);
+  const cudaError_t e = seq == 16 ? launch_seq<16>(tq, tk, tv, p, ctas, stream) : launch_seq<32>(tq, tk, tv, p, ctas, stream);
+  return launched(e, "temporal_attention");
 }
 
 }  // namespace ca

@@ -15,7 +15,6 @@ Stand-alone report:  python -m tests.module_checks [--group adapter|controlnet|u
 from __future__ import annotations
 
 import json
-import os
 import sys
 import time
 
@@ -466,14 +465,33 @@ def check_extra_shapes():
 
 
 def check_controlnet_folded():
-    """ControlNet with CA_FOLD_SMALL_CONV=0: the conditioning-embedding convolutions in their zero-padded form (the
-    folded form -- adjacent pixels in the channel axis -- is the default since round 2 and is what every other ControlNet
-    check exercises)."""
-    os.environ["CA_FOLD_SMALL_CONV"] = "0"
-    try:
-        return check_controlnet(2, 16)
-    finally:
-        os.environ.pop("CA_FOLD_SMALL_CONV", None)
+    """The three convolutions ControlNetConditioningEmbedding folds (adjacent pixels in the channel axis,
+    Conv2d.forward_folded) against their zero-padded form (Conv2d.forward), both on the GPU kernels, at the resolutions
+    of a 512 x 512 control image: conv_in 3 -> 16 on the 8-channel padded image, 16 -> 16 at 512^2, 32 -> 32 at 256^2.
+    Same arithmetic with zeros added, so the two differ by bf16 rounding only (the bound of the CPU test)."""
+    from ctrl_adapter_b200.layers import Conv2d
+    from ctrl_adapter_b200.ops import ACT_SILU
+    torch.manual_seed(0)
+    recs = []
+    for cin, cout, cs, r in ((3, 16, 8, 512), (16, 16, 16, 512), (32, 32, 32, 256)):
+        with torch.device("cuda"), torch.no_grad():
+            conv = Conv2d(cin, cout, 3)
+            conv.bias.normal_(0.0, 0.1)
+            x = torch.zeros(2, r, r, cs)
+            x[..., :cin] = torch.randn(2, r, r, cin)
+        conv = conv.to(BF16).eval()
+        x = x.to(BF16)
+        padded = conv(x, act=ACT_SILU).float()
+        folded = conv.forward_folded(x, act=ACT_SILU).float()
+        torch.cuda.synchronize()
+        err = float((folded - padded).abs().max())
+        bound = 2.0 ** -7 * float(padded.abs().max())
+        fold = conv.fold_factor(x)
+        rec = {"check": f"Conv2d {cin}->{cout} Cs={cs} {r}x{r} SiLU: folded x{fold} vs padded", "max_abs": err,
+               "bound": bound, "ok": fold == 64 // cs and err <= bound}
+        RESULTS.append(rec)
+        recs.append(rec)
+    return recs
 
 
 GROUPS = {

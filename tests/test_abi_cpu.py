@@ -73,6 +73,32 @@ def test_gemm_rejects_blend_with_fp32_output(lib):
     assert b"blend" in lib.ca_last_error()
 
 
+_P = 256  # placeholder device / host pointer: validation fails before anything is dereferenced
+_INVALID_CALLS = [  # entry point, arguments with one out of range, what the message must name
+    ("ca_silu", (_P, 12, _P, None), b"n (12)"),
+    ("ca_add", (_P, _P, 12, _P, None), b"n (12)"),
+    ("ca_upsample2x", (_P, 1, 4, 4, 12, _P, None), b"c (12)"),
+    ("ca_avgpool", (_P, 1, 10, 8, 8, 4, 4, _P, None), b"oh, ow"),
+    ("ca_router_weights", (_P, _P, 1, 33, _P, None), b"nexperts"),
+    ("ca_router_merge", (_P, _P, 9, 64, _P, None), b"nactive"),
+    ("ca_softmax_rows", (_P, 1, 6, _P, None), b"cols (6)"),
+    ("ca_layernorm", (_P, 4, 12, 1e-5, _P, _P, None, 0, None, _P, None), b"c (12)"),
+    ("ca_groupnorm_stats", (_P, 40, None, 0, 1, 16, 32, _P, None), b"groups (32)"),
+    ("ca_cfg_euler_v", (_P, _P, _P, 64, _P, 0, 16, _P, 1, _P, _P, None), b"frames"),
+    ("ca_i2vgen_latent_encoder", (_P, 1, 33, 16, 8, _P, _P, None), b"frames"),
+    ("ca_temporal_attention", (_P, _P, _P, 1, 33, 16, 1, 0.125, 64, _P, None), b"frames"),
+    ("ca_frame_conv_small", (_P, 1, 4, 16, 8, 5, 3, _P, None, _P, None), b"cin"),
+]
+
+
+@pytest.mark.parametrize("name,args,names", _INVALID_CALLS, ids=[c[0] for c in _INVALID_CALLS])
+def test_entry_point_rejects_invalid_argument(lib, name, args, names):
+    """Every entry point checks its arguments before any CUDA call: an out-of-range one returns CA_ERR_INVALID (Python
+    raises ValueError) with a message naming it, with or without a GPU."""
+    assert getattr(lib, name)(*args) == 1
+    assert names in lib.ca_last_error()
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "ctrl_adapter_b200")
     for f in os.listdir(pkg):

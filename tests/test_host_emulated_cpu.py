@@ -92,8 +92,8 @@ def test_emulated_controlnet():
 
 
 def test_emulated_controlnet_folded_small_convs(monkeypatch):
-    """CA_FOLD_SMALL_CONV=1: the 8 / 16 / 32-channel stride-1 convolutions of the conditioning embedding run with adjacent
-    pixels folded into the channel axis (block-banded weights); the ControlNet output must not change."""
+    """The 8 / 16 / 32-channel stride-1 convolutions of the conditioning embedding run with adjacent pixels folded into
+    the channel axis (block-banded weights); the ControlNet output must not change."""
     from ctrl_adapter_b200.controlnet import ControlNetModel
     from ctrl_adapter_b200.layers import Conv2d
     from oracle.controlnet import ControlNetModel as O
@@ -106,7 +106,6 @@ def test_emulated_controlnet_folded_small_convs(monkeypatch):
         calls.append((self.cin, self.cout, self.fold_factor(x)))
         return orig(self, x, **kw)
     monkeypatch.setattr(Conv2d, "forward_folded", spy)
-    monkeypatch.setenv("CA_FOLD_SMALL_CONV", "1")
     _compare(o, p, inputs)
     assert (3, 16, 8) in calls and (16, 16, 4) in calls and (32, 32, 2) in calls, calls
     # and layer-level: folded == unfolded to bf16 rounding on a ragged-free random case

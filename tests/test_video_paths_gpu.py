@@ -1,5 +1,6 @@
 """pytest -m gpu: Stable-Video-Diffusion UNet, the SVD denoising loop (ca_cfg_euler_v), the sparse key-frame path of the
-I2VGen-XL loop, the SVD-geometry kernel shapes and the folded conditioning convolutions -- against the oracle.
+I2VGen-XL loop and the SVD-geometry kernel shapes against the oracle; the folded conditioning convolutions against their
+zero-padded form.
 
 A failure here is red like any other test (nothing is xfail-guarded)."""
 import json
