@@ -90,6 +90,7 @@ SIGNATURES = {
     "ca_cfg_ddim": [_P, _P, _P, _L, _F, _P, _I, _I, _P, _P, _P],
     "ca_i2vgen_latent_encoder": [_P, _I, _I, _L, _I, _P, _P, _P],
     "ca_temporal_attention": [_P, _P, _P, _I, _I, _L, _I, _F, _L, _P, _P],
+    "ca_vae_latents": [_P, _P, _I, _L, _I, _I, _I, _I, _F, _P, _P],
 }
 _RESTYPES = {"ca_last_error": C.c_char_p}
 

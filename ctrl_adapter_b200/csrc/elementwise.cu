@@ -646,4 +646,84 @@ extern "C" int ca_softmax_rows(const float* x, int64_t rows, int64_t cols, void*
                   "softmax_rows");
 }
 
+// ---------------------------------------------------------------------------------------------
+// VAE encoder posterior -> image latents (diffusers DiagonalGaussianDistribution on the quant_conv output, then the
+// image-latent assembly of the two video pipelines).  moments: channels-last bf16 [n, hw, 8] = (mean[4], logvar[4]);
+// noise: optional fp32 NCHW [n, 4, hw].  v = mean + exp(0.5 * clamp(logvar, -30, 20)) * noise (v = mean without noise),
+// fp32, one rounding to bf16 at the store.  One thread per (output batch row, pixel): it reads one 16-byte moment
+// vector and writes its 4 channels into every frame the row has.
+//   CA_VAE_POSTERIOR  out [n, 4, hw]: v
+//   CA_VAE_I2VGEN     out [2*n*nv, 4, F, hw]: frame 0 = v * scale, frame k >= 1 = k / (F - 1); row r holds image r % n
+//   CA_VAE_SVD        out [2*n*nv, F, 4, hw]: row r holds 0 when r % 2n < n, else image r % 2n - n (every frame)
+// ---------------------------------------------------------------------------------------------
+__global__ void vae_latents_kernel(const uint4* __restrict__ moments, const float* __restrict__ noise, int n,
+                                   long long hw, int layout, int frames, long long rows, float scale,
+                                   __nv_bfloat16* __restrict__ out) {
+  CA_PDL_TRIGGER();
+  CA_PDL_WAIT();
+  const long long total = rows * hw;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long p = i % hw, r = i / hw;
+    long long img = r % n;
+    bool zero = false;
+    if (layout == CA_VAE_SVD) {
+      const long long q = r % (2LL * n);
+      zero = q < n;
+      img = zero ? 0 : q - n;
+    }
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (!zero) {
+      const uint4 u = moments[img * hw + p];
+      const float mean[4] = {bf16lo_to_float(u.x), bf16hi_to_float(u.x), bf16lo_to_float(u.y), bf16hi_to_float(u.y)};
+      const float logvar[4] = {bf16lo_to_float(u.z), bf16hi_to_float(u.z), bf16lo_to_float(u.w), bf16hi_to_float(u.w)};
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        v[c] = mean[c];
+        if (noise != nullptr) {
+          const float std = expf(0.5f * fminf(fmaxf(logvar[c], -30.f), 20.f));
+          v[c] = fmaf(std, noise[(img * 4 + c) * hw + p], mean[c]);
+        }
+      }
+    }
+    if (layout == CA_VAE_I2VGEN) {
+      __nv_bfloat16* o = out + r * 4LL * frames * hw + p;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        o[static_cast<long long>(c) * frames * hw] = __float2bfloat16_rn(v[c] * scale);
+        for (int f = 1; f < frames; ++f)
+          o[(static_cast<long long>(c) * frames + f) * hw] =
+              __float2bfloat16_rn(static_cast<float>(f) / static_cast<float>(frames - 1));
+      }
+    } else {
+      // CA_VAE_POSTERIOR has frames == 1: both layouts are [row, frame, channel, pixel]
+      for (int f = 0; f < frames; ++f) {
+        __nv_bfloat16* o = out + (r * frames + f) * 4LL * hw + p;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) o[c * hw] = __float2bfloat16_rn(v[c]);
+      }
+    }
+  }
+}
+extern "C" int ca_vae_latents(const void* moments, const float* noise, int32_t n, int64_t hw, int32_t latent_channels,
+                              int32_t layout, int32_t frames, int32_t num_videos, float scale, void* out, void* s) {
+  if (moments == nullptr) return fail(CA_ERR_INVALID, "vae_latents: null moments pointer");
+  if (out == nullptr) return fail(CA_ERR_INVALID, "vae_latents: null out pointer");
+  if (latent_channels != 4)
+    return fail(CA_ERR_INVALID, "vae_latents: latent_channels (%d) must be 4 (moments carry 8 channels)", latent_channels);
+  if (layout < CA_VAE_POSTERIOR || layout > CA_VAE_SVD)
+    return fail(CA_ERR_INVALID, "vae_latents: layout (%d) must be 0, 1 or 2", layout);
+  if (n < 1 || hw < 1) return fail(CA_ERR_INVALID, "vae_latents: n, hw (%d, %lld) must be positive", n, (long long)hw);
+  if (frames < 1) return fail(CA_ERR_INVALID, "vae_latents: frames (%d) must be positive", frames);
+  if (num_videos < 1) return fail(CA_ERR_INVALID, "vae_latents: num_videos (%d) must be positive", num_videos);
+  if (layout == CA_VAE_POSTERIOR && (frames != 1 || num_videos != 1))
+    return fail(CA_ERR_INVALID, "vae_latents: frames, num_videos (%d, %d) must be 1 for the posterior layout", frames,
+                num_videos);
+  const long long rows = layout == CA_VAE_POSTERIOR ? n : 2LL * n * num_videos;
+  return launched(launch_pdl(vae_latents_kernel, blocks_for(rows * hw, 256), 256, 0, static_cast<cudaStream_t>(s),
+                             static_cast<const uint4*>(moments), noise, n, hw, layout, frames, rows, scale,
+                             static_cast<__nv_bfloat16*>(out)),
+                  "vae_latents");
+}
+
 }  // namespace ca

@@ -75,11 +75,14 @@ class Linear(Packable):
 
 
 class Conv2d(Packable):
-    """3x3 / 1x1 convolution container (PyTorch weight layout [Cout, Cin, k, k])."""
+    """3x3 / 1x1 convolution container (PyTorch weight layout [Cout, Cin, k, k]).  `pad` None: (k-1)/2 zeros on every
+    side; (0, 1) with stride 2: one zero row / column after the bottom / right edge only (diffusers Downsample2D with
+    padding=0, the VAE encoder's down-sampler)."""
 
-    def __init__(self, i: int, o: int, k: int = 3, stride: int = 1):
+    def __init__(self, i: int, o: int, k: int = 3, stride: int = 1, pad: Optional[tuple] = None):
         super().__init__()
         self.k, self.stride, self.cin, self.cout = k, stride, i, o
+        self.pad = pad
         self.weight = nn.Parameter(torch.empty(o, i, k, k))
         self.bias = nn.Parameter(torch.zeros(o))
         nn.init.normal_(self.weight, std=1.0 / math.sqrt(i * k * k))
@@ -94,6 +97,8 @@ class Conv2d(Packable):
 
     def forward(self, x, x2=None, **kw):
         w, b = self.packed()
+        if self.pad is not None:
+            kw["pad"] = self.pad
         return ops.conv2d(x, w, b, ksize=self.k, stride=self.stride, x2=x2, **kw)
 
     # ---- small-channel 3x3 convolutions: fold F adjacent pixels of a row into the channel axis ----------------------

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import torch
 
@@ -239,11 +239,17 @@ def conv2d(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor]
            x2: Optional[torch.Tensor] = None, act: int = ACT_NONE, out_scale: float = 1.0,
            rowvec: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
            blend_src: Optional[torch.Tensor] = None, blend_alpha: Optional[torch.Tensor] = None,
-           out: Optional[torch.Tensor] = None, out_fp32: bool = False, bn: int = 0, k_per_tap: Optional[int] = None):
+           out: Optional[torch.Tensor] = None, out_fp32: bool = False, bn: int = 0, k_per_tap: Optional[int] = None,
+           pad: Optional[Tuple[int, int]] = None):
     """Channels-last conv: x [N,H,W,C] (+ optional x2 [N,H,W,C2] concatenated on C), w_packed [Cout, taps*Kp].
     ksize 1 or 3 (padding (ksize-1)/2), stride 1 or 2 (3x3 only).  rowvec [N, Cout] is broadcast per sample
-    (time-embedding add); residual / blend_src are [N, Ho, Wo, Cout]."""
+    (time-embedding add); residual / blend_src are [N, Ho, Wo, Cout].
+    pad: zero padding (before, after) of both spatial axes; None is (ksize-1)/2 on every side.  Stride 2 also takes
+    (0, 1): one zero row / column at the bottom / right only (diffusers Downsample2D(padding=0) of the VAE encoder)."""
     _req(x); _req(w_packed)
+    if pad is not None and tuple(pad) != (ksize // 2, ksize // 2) and not (stride == 2 and tuple(pad) == (0, 1)):
+        raise ValueError(f"conv2d: pad {tuple(pad)} is not supported at ksize {ksize}, stride {stride}")
+    pad_after_only = pad is not None and tuple(pad) == (0, 1)
     n, h, w_, c = x.shape
     c2 = 0
     if x2 is not None:
@@ -286,10 +292,12 @@ def conv2d(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor]
         d.a_strides[0][0], d.a_strides[0][1], d.a_strides[0][2], d.a_strides[0][3] = 2 * c, w_ * c, 2 * w_ * c, h * w_ * c
         d.box[0], d.box[1], d.box[2], d.box[3] = bw, 1, bh, bnn
         d.ntaps = 9
+        # input row 2*oy + dy - 1: dy=0 -> (parity 1, oy-1); dy=1 -> (0, oy); dy=2 -> (1, oy).
+        # pad (0, 1): input row 2*oy + dy: dy=0 -> (0, oy); dy=1 -> (1, oy); dy=2 -> (0, oy+1), zero filled at oy+1 = H/2
+        taps = ((0, 0), (1, 0), (0, 1)) if pad_after_only else ((1, -1), (0, 0), (1, 0))
         for t, (dy, dx) in enumerate(_TAPS_3X3):
-            # input row 2*oy + dy - 1: dy=0 -> (parity 1, oy-1); dy=1 -> (0, oy); dy=2 -> (1, oy)
-            py, oyo = ((1, -1), (0, 0), (1, 0))[dy]
-            px, oxo = ((1, -1), (0, 0), (1, 0))[dx]
+            py, oyo = taps[dy]
+            px, oxo = taps[dx]
             d.tap_off[t][0], d.tap_off[t][1], d.tap_off[t][2], d.tap_off[t][3] = oxo, py, oyo, 0
             d.tap_c_off[t] = px * c
         d.out_dims[0], d.out_dims[1], d.out_dims[2], d.out_dims[3] = wo, 1, ho, n
@@ -611,3 +619,30 @@ def i2vgen_latent_encoder(x: torch.Tensor, clips: int, frames: int, params: torc
     _launch("i2vgen_latent_encoder", 0.0, 4.0 * x.numel(), "ca_i2vgen_latent_encoder", x.data_ptr(), clips, frames,
             h * w_, cs, params.data_ptr(), y.data_ptr(), _stream())
     return y
+
+
+VAE_POSTERIOR, VAE_I2VGEN, VAE_SVD = 0, 1, 2
+
+
+def vae_latents(moments: torch.Tensor, layout: int = VAE_POSTERIOR, noise: Optional[torch.Tensor] = None,
+                frames: int = 1, num_videos: int = 1, scale: float = 1.0):
+    """VAE posterior -> latents (layouts: include/ctrl_adapter_b200.h ``ca_vae_latents``).  moments [n, h, w, 8] bf16
+    (mean, logvar); noise fp32 [n, 4, h, w] or None (the posterior's mode).  Returns bf16
+    VAE_POSTERIOR [n, 4, h, w] / VAE_I2VGEN [2*n*nv, 4, F, h, w] / VAE_SVD [2*n*nv, F, 4, h, w]."""
+    _req(moments)
+    n, h, w_, cm = moments.shape
+    if cm != 8:
+        raise ValueError(f"vae_latents: moments carry {cm} channels, expected 8 (mean and logvar of 4 latent channels)")
+    if noise is not None:
+        _req(noise, torch.float32)
+        if tuple(noise.shape) != (n, 4, h, w_):
+            raise ValueError(f"vae_latents: noise shape {tuple(noise.shape)}, expected {(n, 4, h, w_)}")
+    rows = n if layout == VAE_POSTERIOR else 2 * n * num_videos
+    shape = {VAE_POSTERIOR: (n, 4, h, w_), VAE_I2VGEN: (rows, 4, frames, h, w_),
+             VAE_SVD: (rows, frames, 4, h, w_)}.get(layout)
+    if shape is None or min(shape) < 1:
+        raise ValueError(f"vae_latents: layout {layout}, frames {frames}, num_videos {num_videos}")
+    out = torch.empty(shape, device=moments.device, dtype=BF16)
+    _launch("vae_latents", 0.0, 2.0 * (moments.numel() + out.numel()), "ca_vae_latents", moments.data_ptr(),
+            _ptr(noise), n, h * w_, 4, layout, frames, num_videos, float(scale), out.data_ptr(), _stream())
+    return out

@@ -13,7 +13,12 @@ objects it was constructed with (e.g. the diffusers / transformers ones where th
 absent the caller passes that stage's OUTPUT instead -- ``prompt_embeds`` ... exactly as the reference signature already
 allows, plus the keyword-only extensions listed in each ``__call__`` (``controlnet_prompt_embeds``, ``image_embeddings``,
 ``image_latents``, tensor ``control_images``).  ``output_type="latent"`` needs no VAE; with
-``vae=ctrl_adapter_b200.vae.AutoencoderKL`` the SDXL and I2VGen-XL pipelines decode on the H100 kernels as well.  Nothing
+``vae=ctrl_adapter_b200.vae.AutoencoderKL`` the SDXL and I2VGen-XL pipelines decode on the H100 kernels as well.
+The two video pipelines also take the reference's ``image=`` (a PIL image, a list of them, or a [N, 3, H, W] tensor in
+[0, 1]): the image latents are then built with ``self.vae.encode`` (our ``AutoencoderKL`` /
+``AutoencoderKLTemporalDecoder`` on the H100 kernels, or any object with diffusers' ``encode()`` / ``config``) and the
+image embeddings with the ``image_encoder`` + ``feature_extractor`` components, after the reference's own crop / resize
+preprocessing (``encode_image`` of each pipeline).  Passed ``image_latents`` / ``image_embeddings`` keep priority.  Nothing
 here falls back to a PyTorch implementation of the hot path.
 """
 from __future__ import annotations
@@ -24,11 +29,12 @@ from typing import Any, Callable, Dict, List, Optional, Tuple, Union
 
 import torch
 
+from . import ops
 from .controlnet import MultiControlNetModel
 from .pipeline_i2vgen import I2VGenXLControlNetAdapterLoop
 from .pipeline_sdxl import SDXLControlNetAdapterLoop
 from .pipeline_svd import SVDControlNetAdapterLoop
-from .vae import decode_latents, svd_decode_latents, tensor2vid
+from .vae import DiagonalGaussianDistribution, decode_latents, svd_decode_latents, tensor2vid
 from .vae import postprocess as vae_postprocess
 
 BF16 = torch.bfloat16
@@ -166,6 +172,138 @@ def _vae(pipe):
     return _need(getattr(pipe, "vae", None), "a `vae` component (or output_type='latent')", "VAE")
 
 
+# ---- conditioning-image preprocessing of the two video pipelines (restated from the reference and diffusers'
+# VaeImageProcessor; i2vgen pipeline :1150-1203, svd pipeline :165-193, utils/utils_svd.py _resize_with_antialiasing) ----
+def _image_list(image) -> list:
+    """PIL image / list of them / [n, 3, H, W] (or [3, H, W]) tensor in [0, 1] -> list of PIL images"""
+    from PIL import Image
+    if isinstance(image, Image.Image):
+        return [image]
+    if torch.is_tensor(image):
+        t = image.unsqueeze(0) if image.dim() == 3 else image
+        arr = (t.detach().float().cpu().permute(0, 2, 3, 1).numpy() * 255).round().astype("uint8")
+        return [Image.fromarray(a) for a in arr]
+    if isinstance(image, (list, tuple)) and len(image) > 0:
+        return [im for x in image for im in _image_list(x)]
+    raise ValueError(f"`image` has to be a PIL image, a list of PIL images or a [N, 3, H, W] tensor, got {type(image)}")
+
+
+def _center_crop_wide(image, resolution: Tuple[int, int]):
+    """Resize (PIL BOX) so that the image covers `resolution` = (W, H) -- scale = min(w / W, h / H) of the first image,
+    sizes round(w // scale) x round(h // scale) -- then crop the centred W x H box.  Tensors are converted to PIL first;
+    a list comes back as a list."""
+    from PIL import Image
+    single = not isinstance(image, (list, tuple)) and not (torch.is_tensor(image) and image.dim() == 4)
+    ims = _image_list(image)
+    scale = min(ims[0].size[0] / resolution[0], ims[0].size[1] / resolution[1])
+    ims = [u.resize((round(u.width // scale), round(u.height // scale)), resample=Image.BOX) for u in ims]
+    x1, y1 = (ims[0].width - resolution[0]) // 2, (ims[0].height - resolution[1]) // 2
+    ims = [u.crop((x1, y1, x1 + resolution[0], y1 + resolution[1])) for u in ims]
+    return ims[0] if single else ims
+
+
+def _resize_bilinear(image, resolution: Tuple[int, int]):
+    from PIL import Image
+    if isinstance(image, (list, tuple)):
+        return [u.resize(resolution, Image.BILINEAR) for u in image]
+    return image.resize(resolution, Image.BILINEAR)
+
+
+def _pil_to_pt(images) -> torch.Tensor:
+    """VaeImageProcessor.pil_to_numpy + numpy_to_pt: list of PIL -> [n, 3, H, W] fp32 in [0, 1]"""
+    import numpy as np
+    images = images if isinstance(images, (list, tuple)) else [images]
+    arr = np.stack([np.array(im).astype(np.float32) / 255.0 for im in images])
+    return torch.from_numpy(arr.transpose(0, 3, 1, 2))
+
+
+def _vae_preprocess(image, height: Optional[int] = None, width: Optional[int] = None) -> torch.Tensor:
+    """VaeImageProcessor.preprocess with do_normalize: PIL images are resized (Lanczos) to height x width when given,
+    tensors in [0, 1] (nearest); then 2x - 1.  A tensor that already has negative values is taken as normalised."""
+    from .helper import ControlNetHelper
+    if torch.is_tensor(image):
+        t = image.float().unsqueeze(0) if image.dim() == 3 else image.float()
+        h, w = (height or t.shape[-2]), (width or t.shape[-1])
+        t = ControlNetHelper._preprocess(t, h, w)
+        return t if float(t.min()) < 0 else 2.0 * t - 1.0
+    ims = _image_list(image)
+    out = [ControlNetHelper._preprocess(im, height or im.height, width or im.width) for im in ims]
+    return 2.0 * torch.cat(out) - 1.0
+
+
+def _gaussian_window(size: int, sigma: float) -> torch.Tensor:
+    x = torch.arange(size, dtype=torch.float32) - size // 2
+    if size % 2 == 0:
+        x = x + 0.5
+    g = torch.exp(-x.pow(2.0) / (2 * sigma ** 2))
+    return g / g.sum()
+
+
+def _resize_with_antialiasing(x: torch.Tensor, size: Tuple[int, int]) -> torch.Tensor:
+    """[n, C, H, W] fp32 -> [n, C, size]: separable Gaussian blur (sigma = max((factor - 1) / 2, 0.001) per axis, odd
+    window of int(max(4 sigma, 3)) taps, reflect padding), then bicubic interpolation with align_corners=True -- the
+    anti-aliased down-sizing the SVD pipeline applies before the CLIP image encoder."""
+    import torch.nn.functional as F
+    h, w = x.shape[-2:]
+    sig = (max((h / size[0] - 1.0) / 2.0, 0.001), max((w / size[1] - 1.0) / 2.0, 0.001))
+    ks = [int(max(2.0 * 2 * s, 3)) for s in sig]
+    ks = [k + 1 if k % 2 == 0 else k for k in ks]
+    n, c = x.shape[:2]
+    for axis, (k, s) in ((1, (ks[1], sig[1])), (0, (ks[0], sig[0]))):   # x first, then y
+        g = _gaussian_window(k, s).to(device=x.device, dtype=x.dtype)
+        kern = g.view(1, 1, 1, k) if axis == 1 else g.view(1, 1, k, 1)
+        lo = (k - 1) // 2
+        pad = (lo, k - 1 - lo, 0, 0) if axis == 1 else (0, 0, lo, k - 1 - lo)
+        xp = F.pad(x, pad, mode="reflect")
+        x = F.conv2d(xp.reshape(n * c, 1, *xp.shape[-2:]), kern).reshape(n, c, h, w)
+    return F.interpolate(x, size=size, mode="bicubic", align_corners=True)
+
+
+def _clip_image_embeddings(image_encoder, feature_extractor, pixels: torch.Tensor, device, num_videos_per_prompt: int):
+    """CLIP image embeddings as both pipelines' _encode_image builds them: pixels [n, 3, H, W] in [0, 1] -> normalised by
+    the feature extractor -> image_encoder(...).image_embeds -> (2 * n * nv, 1, D), zeros for the unconditional half."""
+    _need(image_encoder, "image_embeddings (or an `image_encoder` component)", "CLIP vision encoder")
+    _need(feature_extractor, "image_embeddings (or a `feature_extractor` component)", "CLIP image processor")
+    pv = feature_extractor(images=pixels, do_normalize=True, do_center_crop=False, do_resize=False, do_rescale=False,
+                           return_tensors="pt").pixel_values
+    dtype = next(image_encoder.parameters()).dtype
+    emb = image_encoder(pv.to(device=device, dtype=dtype)).image_embeds.unsqueeze(1)
+    bs, seq, _ = emb.shape
+    emb = emb.repeat(1, num_videos_per_prompt, 1).view(bs * num_videos_per_prompt, seq, -1)
+    return torch.cat([torch.zeros_like(emb), emb])
+
+
+def _posterior(vae, image: torch.Tensor):
+    return vae.encode(image).latent_dist
+
+
+def i2vgen_image_latents(vae, image: torch.Tensor, num_frames: int, num_videos_per_prompt: int,
+                         noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """i2vgen pipeline :487-517 prepare_image_latents: image [n, 3, H, W] in [-1, 1] -> (2*n*nv, 4, F, h, w) bf16:
+    frame 0 = posterior sample * scaling_factor (noise from the global RNG unless given), frame k = k / (F - 1)."""
+    post = _posterior(vae, image)
+    if isinstance(post, DiagonalGaussianDistribution):
+        return ops.vae_latents(post.moments, ops.VAE_I2VGEN, noise=post.noise() if noise is None else noise,
+                               frames=num_frames, num_videos=num_videos_per_prompt, scale=vae.config.scaling_factor)
+    # a diffusers-compatible VAE: the same assembly on its tensors
+    x = (post.sample() * vae.config.scaling_factor).unsqueeze(2)
+    pos = [torch.ones_like(x) * ((k + 1) / (num_frames - 1)) for k in range(num_frames - 1)]
+    x = torch.cat([x] + pos, dim=2).repeat(num_videos_per_prompt, 1, 1, 1, 1)
+    return torch.cat([x, x]).to(BF16)
+
+
+def svd_image_latents(vae, image: torch.Tensor, num_frames: int, num_videos_per_prompt: int) -> torch.Tensor:
+    """svd pipeline :214-235 _encode_vae_image + :580-583: image [n, 3, H, W] -> (2*n*nv, F, 4, h, w) bf16 = posterior
+    mode (no scaling factor) after zeros, repeated nv times, then over the frames (for nv > 1 the batch order is
+    [0, L, 0, L], the reference's)."""
+    post = _posterior(vae, image)
+    if isinstance(post, DiagonalGaussianDistribution):
+        return ops.vae_latents(post.moments, ops.VAE_SVD, frames=num_frames, num_videos=num_videos_per_prompt)
+    m = post.mode()
+    x = torch.cat([torch.zeros_like(m), m]).repeat(num_videos_per_prompt, 1, 1, 1)
+    return x.unsqueeze(1).repeat(1, num_frames, 1, 1, 1).to(BF16)
+
+
 # ------------------------------------------------------------------------------------------------------------------
 class SDXLControlNetAdapterPipeline(DiffusionPipeline):
     """sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:235-275 (constructor), :829-1434 (__call__)."""
@@ -298,6 +436,28 @@ class I2VGenXLControlNetAdapterPipeline(DiffusionPipeline):
         self.vae_scale_factor = 8
 
     @torch.no_grad()
+    def encode_image(self, image, height: int, width: int, num_frames: int, num_videos_per_prompt: int = 1,
+                     device=None, embeddings: bool = True, latents: bool = True, noise: Optional[torch.Tensor] = None):
+        """The conditioning image as the loop takes it (:795-812): (image_embeddings (2*n*nv, 1, D) or None,
+        image_latents (2*n*nv, 4, F, h, w) bf16 or None) for n images.
+        CLIP: _center_crop_wide to width x width, bilinear resize to the feature extractor's crop size, image_encoder.
+        VAE: _center_crop_wide to width x height, 2x - 1, vae.encode, posterior sample (unit noise from the global RNG,
+        as the reference draws it, unless `noise` [n, 4, h, w] fp32 is given) * scaling_factor, position planes."""
+        device = device or self._execution_device
+        emb = lat = None
+        if embeddings:
+            fe = _need(self.feature_extractor, "image_embeddings (or a `feature_extractor` component)",
+                       "CLIP image processor")
+            crop = fe.crop_size
+            ims = _resize_bilinear(_center_crop_wide(_image_list(image), (width, width)), (crop["width"], crop["height"]))
+            emb = _clip_image_embeddings(self.image_encoder, fe, _pil_to_pt(ims), device, num_videos_per_prompt)
+        if latents:
+            vae = _need(getattr(self, "vae", None), "image_latents (or a `vae` component)", "VAE")
+            x = _vae_preprocess(_center_crop_wide(_image_list(image), (width, height))).to(device=device, dtype=BF16)
+            lat = i2vgen_image_latents(vae, x, num_frames, num_videos_per_prompt, noise)
+        return emb, lat
+
+    @torch.no_grad()
     def __call__(self, prompt: Union[str, List[str]] = None, image=None, height: Optional[int] = 704,
                  width: Optional[int] = 1280, target_fps: Optional[int] = 16, num_frames: int = 16,
                  num_inference_steps: int = 50, guidance_scale: float = 9.0, negative_prompt=None, eta: float = 0.0,
@@ -325,9 +485,15 @@ class I2VGenXLControlNetAdapterPipeline(DiffusionPipeline):
         prompt_embeds = _need(prompt_embeds, "prompt_embeds", "text encoder")
         negative_prompt_embeds = _need(negative_prompt_embeds, "negative_prompt_embeds", "text encoder")
         b = prompt_embeds.shape[0]
-        # image_embeddings (2B,1,1024) negative first (:808-815); image_latents (2B,4,F,h,w) (:818-833)
-        image_embeddings = _need(image_embeddings, "image_embeddings", "CLIP vision encoder").to(device)
-        image_latents = _need(image_latents, "image_latents", "VAE encoder").to(device)
+        # image_embeddings (2B,1,1024) negative first (:808-815); image_latents (2B,4,F,h,w) (:818-833); built from
+        # `image` when not passed
+        if image is not None and (image_embeddings is None or image_latents is None):
+            emb, lat_img = self.encode_image(image, height, width, f, num_videos_per_prompt, device,
+                                             embeddings=image_embeddings is None, latents=image_latents is None)
+            image_embeddings = emb if image_embeddings is None else image_embeddings
+            image_latents = lat_img if image_latents is None else image_latents
+        image_embeddings = _need(image_embeddings, "image_embeddings (or `image`)", "CLIP vision encoder").to(device)
+        image_latents = _need(image_latents, "image_latents (or `image`)", "VAE encoder").to(device)
         if controlnet_prompt_embeds is None:
             helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")
             controlnet_prompt_embeds, controlnet_negative_prompt_embeds, _, _ = helper.encode_controlnet_prompt(
@@ -391,6 +557,33 @@ class SVDControlNetAdapterPipeline(DiffusionPipeline):
         return svd_decode_latents(_vae(self), latents, num_frames, decode_chunk_size)
 
     @torch.no_grad()
+    def encode_image(self, image, height: int, width: int, num_frames: int, num_videos_per_prompt: int = 1,
+                     noise_aug_strength: float = 0.02, generator=None, device=None, embeddings: bool = True,
+                     latents: bool = True):
+        """The conditioning image as the loop takes it (:553-583): (image_embeddings (2*n*nv, 1, D) or None,
+        image_latents (2*n*nv, F, 4, h, w) bf16 or None) for n images.
+        CLIP: 2x - 1, _resize_with_antialiasing to 224 x 224, (x + 1) / 2 (PIL input; a tensor goes to the feature
+        extractor as it is, as in the reference), image_encoder.
+        VAE: Lanczos resize to width x height, 2x - 1, + noise_aug_strength * randn(generator), vae.encode, posterior
+        mode (no scaling factor), zeros for the unconditional half."""
+        device = device or self._execution_device
+        emb = lat = None
+        if embeddings:
+            if torch.is_tensor(image):
+                pixels = image.float().unsqueeze(0) if image.dim() == 3 else image.float()
+            else:
+                pixels = (_resize_with_antialiasing(_pil_to_pt(_image_list(image)) * 2.0 - 1.0, (224, 224)) + 1.0) / 2.0
+            emb = _clip_image_embeddings(self.image_encoder, _need(self.feature_extractor, "image_embeddings (or a "
+                                         "`feature_extractor` component)", "CLIP image processor"), pixels, device,
+                                         num_videos_per_prompt)
+        if latents:
+            vae = _need(getattr(self, "vae", None), "image_latents (or a `vae` component)", "VAE")
+            x = _vae_preprocess(image, height, width).to(device)
+            x = x + noise_aug_strength * _randn(tuple(x.shape), generator, device)
+            lat = svd_image_latents(vae, x, num_frames, num_videos_per_prompt)
+        return emb, lat
+
+    @torch.no_grad()
     def __call__(self, image=None, prompt: str = "", height: int = 576, width: int = 1024,
                  num_frames: Optional[int] = None, num_inference_steps: int = 25, min_guidance_scale: float = 1.0,
                  max_guidance_scale: float = 3.0, fps: int = 7, motion_bucket_id: int = 127,
@@ -415,9 +608,18 @@ class SVDControlNetAdapterPipeline(DiffusionPipeline):
             raise NotImplementedError("Multi-ControlNet / callbacks / guess_mode: not on the SVD inference path")
         device = self._execution_device
         f = num_frames if num_frames is not None else self.unet.config.num_frames
-        # image_embeddings (2B,1,1024): zeros for the unconditional half (:497-503); image_latents (2B,F,4,h,w) (:566-583)
-        image_embeddings = _need(image_embeddings, "image_embeddings", "CLIP vision encoder").to(device)
-        image_latents = _need(image_latents, "image_latents", "VAE encoder").to(device)
+        # image_embeddings (2B,1,1024): zeros for the unconditional half (:497-503); image_latents (2B,F,4,h,w) (:566-583);
+        # built from `image` when not passed.  The noise augmentation draws from `generator` before the latents do.
+        if image is not None and (image_embeddings is None or image_latents is None):
+            emb, lat_img = self.encode_image(image, height, width, f, num_videos_per_prompt, noise_aug_strength,
+                                             generator, device, embeddings=image_embeddings is None,
+                                             latents=image_latents is None)
+            image_embeddings = emb if image_embeddings is None else image_embeddings
+            image_latents = lat_img if image_latents is None else image_latents
+            # B below is image_embeddings.shape[0] // 2, which now counts every video of every image
+            num_videos_per_prompt = 1
+        image_embeddings = _need(image_embeddings, "image_embeddings (or `image`)", "CLIP vision encoder").to(device)
+        image_latents = _need(image_latents, "image_latents (or `image`)", "VAE encoder").to(device)
         b = image_embeddings.shape[0] // 2
         if controlnet_prompt_embeds is None:
             helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")

@@ -1,13 +1,18 @@
-"""H100 host mirror of the decoder half of diffusers' ``AutoencoderKL`` -- the VAE ``decode`` the reference pipelines
-call after the denoising loop (/root/reference/sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1414;
-i2vgen_xl/pipelines/i2vgen_xl_controlnet_adapter_pipeline.py:398-418 ``decode_latents``; SURVEY.md section 8f row 1).
+"""H100 host mirror of diffusers' ``AutoencoderKL`` -- the VAE ``decode`` the reference pipelines call after the
+denoising loop (/root/reference/sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1414;
+i2vgen_xl/pipelines/i2vgen_xl_controlnet_adapter_pipeline.py:398-418 ``decode_latents``; SURVEY.md section 8f row 1)
+and the ``encode`` of the conditioning image before it (i2vgen pipeline :487-517, svd pipeline :214-235; section 8f
+row 2).
 
-Same constructor kwargs, ``decode()`` call form and state-dict keys as the diffusers class (``post_quant_conv.*``,
-``decoder.conv_in / mid_block.{resnets,attentions} / up_blocks.N.{resnets,upsamplers} / conv_norm_out / conv_out``); the
-encoder half (``encoder.*``, ``quant_conv.*``) is not part of the path and its keys are skipped at load time.  Everything
-runs on the kernels of the denoising path: 3x3 / 1x1 convolutions on the implicit-GEMM kernel, GroupNorm(+SiLU) kernels,
-the 2x nearest up-sampler; the mid block's single 512-wide attention head (outside ``attention_kernel``'s head dims, and
-run once per generation) as QK^T GEMM (fp32) -> ``ca_softmax_rows`` -> PV GEMM, one image at a time.
+Same constructor kwargs, ``encode()`` / ``decode()`` call forms and state-dict keys as the diffusers class
+(``encoder.conv_in / down_blocks.N.{resnets,downsamplers} / mid_block / conv_norm_out / conv_out``, ``quant_conv.*``,
+``post_quant_conv.*``, ``decoder.conv_in / mid_block.{resnets,attentions} / up_blocks.N.{resnets,upsamplers} /
+conv_norm_out / conv_out``).  A checkpoint without a complete encoder half still loads its decoder (see ``_KLVae``).
+Everything runs on the kernels of the denoising path: 3x3 / 1x1 convolutions on the implicit-GEMM kernel (the encoder's
+down-samplers on its stride-2 parity view with bottom / right padding), GroupNorm(+SiLU) kernels, the 2x nearest
+up-sampler; the mid block's single 512-wide attention head (outside ``attention_kernel``'s head dims, and run once per
+generation) as QK^T GEMM (fp32) -> ``ca_softmax_rows`` -> PV GEMM, one image at a time; the posterior and the pipelines'
+image-latent layouts in ``ca_vae_latents``.
 
 ``AutoencoderKLTemporalDecoder`` (decoder half) is the VAE of the SVD pipeline (svd/pipelines/
 svd_controlnet_adapter_pipeline.py:265-292 ``decode_latents``): every decoder ResNet is a SpatioTemporalResBlock (spatial
@@ -127,8 +132,114 @@ class DecoderOutput:
         self.sample = sample
 
 
-class _DecoderOnlyVae(PretrainedMixin, nn.Module):
-    ignore_prefixes = ("encoder.", "quant_conv.")  # the encoder half of a published checkpoint is not on the path
+# ---- encoder half (diffusers v0.27.2 models/autoencoders/vae.py Encoder with double_z=True) ---------------------------
+class _DownEncoderBlock(nn.Module):
+    """diffusers DownEncoderBlock2D: resnets (eps 1e-6, no time embedding), then Downsample2D(padding=0) -- a 3x3
+    stride-2 convolution after one zero row / column at the bottom / right -- on every block but the last."""
+
+    def __init__(self, cin: int, cout: int, layers: int, eps: float, add_downsample: bool):
+        super().__init__()
+        self.resnets = nn.ModuleList([ResnetBlock2D(cin if i == 0 else cout, cout, None, eps) for i in range(layers)])
+        self.downsamplers = None
+        if add_downsample:
+            ds = nn.Module()
+            ds.conv = Conv2d(cout, cout, 3, stride=2, pad=(0, 1))
+            self.downsamplers = nn.ModuleList([ds])
+
+    def forward(self, x):
+        for r in self.resnets:
+            x = r(x, None)
+        if self.downsamplers is not None:
+            x = self.downsamplers[0].conv(x)
+        return x
+
+
+class Encoder(nn.Module):
+    """conv_in -> down blocks -> mid block (2 resnets + the single-head attention) -> GroupNorm + SiLU -> conv_out with
+    2 * latent_channels outputs: the mean and log-variance of the diagonal Gaussian posterior."""
+
+    def __init__(self, in_channels: int, latent_channels: int, block_out_channels, layers_per_block: int, eps: float):
+        super().__init__()
+        self.conv_in = Conv2d(in_channels, block_out_channels[0], 3)
+        blocks, prev = [], block_out_channels[0]
+        for i, c in enumerate(block_out_channels):
+            blocks.append(_DownEncoderBlock(prev, c, layers_per_block, eps, i != len(block_out_channels) - 1))
+            prev = c
+        self.down_blocks = nn.ModuleList(blocks)
+        self.mid_block = _MidBlock(block_out_channels[-1], eps)
+        self.conv_norm_out = Norm(block_out_channels[-1], eps)
+        self.conv_out = Conv2d(block_out_channels[-1], 2 * latent_channels, 3)
+
+    def forward(self, x_nhwc8):
+        x = self.conv_in(x_nhwc8)
+        for blk in self.down_blocks:
+            x = blk(x)
+        x = self.mid_block(x)
+        x = self.conv_norm_out.group_norm(x, silu=True)
+        return self.conv_out(x)  # [n, h, w, 2 * latent_channels]
+
+
+class DiagonalGaussianDistribution:
+    """diffusers DiagonalGaussianDistribution over the quant_conv output: mean = channels 0-3, logvar = channels 4-7
+    clamped to [-30, 20].  ``mode()`` / ``sample()`` run ``ca_vae_latents``; the result is bf16 [n, 4, h, w]."""
+
+    def __init__(self, moments: torch.Tensor):
+        self.moments = moments  # [n, h, w, 8] bf16, channels-last
+        self.deterministic = False
+
+    @property
+    def mean(self):
+        return self.mode()
+
+    @property
+    def logvar(self):
+        return self.moments[..., 4:].permute(0, 3, 1, 2).float().clamp(-30.0, 20.0).to(self.moments.dtype)
+
+    @property
+    def std(self):
+        return torch.exp(0.5 * self.logvar.float()).to(self.moments.dtype)
+
+    @property
+    def var(self):
+        return torch.exp(self.logvar.float()).to(self.moments.dtype)
+
+    def mode(self):
+        return ops.vae_latents(self.moments, ops.VAE_POSTERIOR)
+
+    def noise(self, generator=None):
+        """The unit noise ``sample(generator)`` uses: drawn as diffusers' randn_tensor draws it (the posterior's shape and
+        dtype, on the generator's device, the global RNG when generator is None), as fp32 on the moments' device."""
+        n, h, w, _ = self.moments.shape
+        if isinstance(generator, (list, tuple)):
+            generator = generator[0]
+        dev = generator.device if generator is not None else self.moments.device
+        return torch.randn((n, 4, h, w), generator=generator, device=dev, dtype=self.moments.dtype).to(
+            self.moments.device, torch.float32)
+
+    def sample(self, generator=None, noise: Optional[torch.Tensor] = None):
+        """mean + std * noise; `noise` (fp32 [n, 4, h, w]) replaces the draw."""
+        return ops.vae_latents(self.moments, ops.VAE_POSTERIOR, noise=self.noise(generator) if noise is None else noise)
+
+
+class AutoencoderKLOutput:
+    def __init__(self, latent_dist):
+        self.latent_dist = latent_dist
+
+
+class _KLVae(PretrainedMixin, nn.Module):
+    """What the two VAEs share: the encoder half, its loading rules and ``encode()``.
+
+    A published checkpoint carries both halves.  The encoder half (``encoder.*``, ``quant_conv.*``) is loaded only when
+    the state dict carries every one of its keys with the module's shapes; otherwise those keys are skipped, the decoder
+    half loads as before, and ``encode()`` raises until a complete encoder is loaded.  A freshly constructed module can
+    encode (with its random weights)."""
+
+    encoder_prefixes = ("encoder.", "quant_conv.")
+
+    def _init_encoder(self, in_channels, latent_channels, block_out_channels, layers_per_block):
+        self.encoder = Encoder(in_channels, latent_channels, block_out_channels, layers_per_block, 1e-6)
+        self.quant_conv = Conv2d(2 * latent_channels, 2 * latent_channels, 1)
+        self.encoder_loaded = True
 
     @property
     def dtype(self):
@@ -139,24 +250,55 @@ class _DecoderOnlyVae(PretrainedMixin, nn.Module):
         return next(self.parameters()).device
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
-        sd = {k: v for k, v in state_dict.items() if not k.startswith(self.ignore_prefixes)}
-        return super().load_state_dict(sd, strict=strict, **kw)
+        own = {k: tuple(v.shape) for k, v in self.state_dict().items() if k.startswith(self.encoder_prefixes)}
+        complete = all(k in state_dict and tuple(state_dict[k].shape) == s for k, s in own.items())
+        if complete:
+            res = super().load_state_dict(state_dict, strict=strict, **kw)
+            self.encoder_loaded = True
+            return res
+        sd = {k: v for k, v in state_dict.items() if not k.startswith(self.encoder_prefixes)}
+        res = super().load_state_dict(sd, strict=False, **kw)
+        missing = [k for k in res.missing_keys if not k.startswith(self.encoder_prefixes)]
+        if strict and (missing or res.unexpected_keys):
+            raise RuntimeError(f"Error(s) in loading state_dict for {type(self).__name__}: missing keys {missing}, "
+                               f"unexpected keys {res.unexpected_keys}")
+        self.encoder_loaded = False
+        return type(res)(missing, res.unexpected_keys)
+
+    @torch.no_grad()
+    def encode(self, x: torch.Tensor, return_dict: bool = True):
+        """x [N, 3, H, W] in [-1, 1] (fp32 or bf16, H and W multiples of 8) -> AutoencoderKLOutput(latent_dist=
+        DiagonalGaussianDistribution) over [N, 4, H/8, W/8] latents."""
+        if not self.encoder_loaded:
+            raise ValueError(f"{type(self).__name__}.encode: the encoder weights were not loaded (the state dict did not "
+                             f"carry a complete encoder.* / quant_conv.* set); load a full checkpoint to encode")
+        f = 2 ** (len(self.config.block_out_channels) - 1)
+        if x.dim() != 4 or x.shape[1] != self.config.in_channels:
+            raise ValueError(f"encode expects [N, {self.config.in_channels}, H, W] images, got {tuple(x.shape)}")
+        if x.shape[2] % f or x.shape[3] % f:
+            raise ValueError(f"`height` and `width` have to be divisible by {f} but are {x.shape[2]} and {x.shape[3]}.")
+        x = to_channels_last_bf16(x.to(self.device), 8)  # 3 -> 8 zero-padded channels
+        moments = self.quant_conv(self.encoder(x))     # [N, h, w, 8] = (mean, logvar)
+        post = DiagonalGaussianDistribution(moments)
+        return AutoencoderKLOutput(post) if return_dict else (post,)
 
 
-class AutoencoderKL(_DecoderOnlyVae):
+class AutoencoderKL(_KLVae):
 
     def __init__(self, in_channels: int = 3, out_channels: int = 3, down_block_types=("DownEncoderBlock2D",) * 4,
                  up_block_types=("UpDecoderBlock2D",) * 4, block_out_channels=(128, 256, 512, 512),
                  layers_per_block: int = 2, act_fn: str = "silu", latent_channels: int = 4, norm_num_groups: int = 32,
                  sample_size: int = 1024, scaling_factor: float = 0.13025, force_upcast: bool = True, **_ignored):
         super().__init__()
-        if act_fn != "silu" or norm_num_groups != 32 or any(t != "UpDecoderBlock2D" for t in up_block_types):
-            raise NotImplementedError("only the SD / SDXL AutoencoderKL decoder topology is implemented")
+        if act_fn != "silu" or norm_num_groups != 32 or any(t != "UpDecoderBlock2D" for t in up_block_types) or \
+                any(t != "DownEncoderBlock2D" for t in down_block_types):
+            raise NotImplementedError("only the SD / SDXL AutoencoderKL topology is implemented")
         self.config = _ConfigDict(in_channels=in_channels, out_channels=out_channels,
                                   down_block_types=tuple(down_block_types), up_block_types=tuple(up_block_types),
                                   block_out_channels=tuple(block_out_channels), layers_per_block=layers_per_block,
                                   act_fn=act_fn, latent_channels=latent_channels, norm_num_groups=norm_num_groups,
                                   sample_size=sample_size, scaling_factor=scaling_factor, force_upcast=force_upcast)
+        self._init_encoder(in_channels, latent_channels, block_out_channels, layers_per_block)
         self.post_quant_conv = Conv2d(latent_channels, latent_channels, 1)
         self.decoder = Decoder(latent_channels, out_channels, block_out_channels, layers_per_block, 1e-6)
 
@@ -279,11 +421,10 @@ class TemporalDecoder(nn.Module):
         return self.time_conv_out(y, frames)
 
 
-class AutoencoderKLTemporalDecoder(_DecoderOnlyVae):
-    """Decoder half of the SVD VAE (stabilityai/stable-video-diffusion-img2vid[-xt] ``vae``): same constructor kwargs,
-    ``decode(z, num_frames)`` call form and ``decoder.*`` state-dict keys as the diffusers class.  There is no
-    post_quant_conv in this model; ``encoder.*`` / ``quant_conv.*`` keys of a checkpoint are skipped (the conditioning
-    image is encoded once per call, outside the path)."""
+class AutoencoderKLTemporalDecoder(_KLVae):
+    """The SVD VAE (stabilityai/stable-video-diffusion-img2vid[-xt] ``vae``): same constructor kwargs,
+    ``encode(x)`` / ``decode(z, num_frames)`` call forms and state-dict keys as the diffusers class.  Its encoder is the
+    2-D ``Encoder`` of AutoencoderKL (with quant_conv); there is no post_quant_conv in this model."""
 
     def __init__(self, in_channels: int = 3, out_channels: int = 3, down_block_types=("DownEncoderBlock2D",) * 4,
                  block_out_channels=(128, 256, 512, 512), layers_per_block: int = 2, latent_channels: int = 4,
@@ -293,6 +434,9 @@ class AutoencoderKLTemporalDecoder(_DecoderOnlyVae):
                                   down_block_types=tuple(down_block_types), block_out_channels=tuple(block_out_channels),
                                   layers_per_block=layers_per_block, latent_channels=latent_channels,
                                   sample_size=sample_size, scaling_factor=scaling_factor, force_upcast=force_upcast)
+        if any(t != "DownEncoderBlock2D" for t in down_block_types):
+            raise NotImplementedError("only the SVD AutoencoderKLTemporalDecoder topology is implemented")
+        self._init_encoder(in_channels, latent_channels, block_out_channels, layers_per_block)
         self.decoder = TemporalDecoder(latent_channels, out_channels, block_out_channels, layers_per_block)
 
     @torch.no_grad()

@@ -211,6 +211,24 @@ int ca_i2vgen_latent_encoder(const void* x, int32_t clips, int32_t frames, int64
                              const float* params, void* y, void* cuda_stream);
 
 /*
+ * VAE encoder posterior and image-latent assembly: diffusers DiagonalGaussianDistribution on the quant_conv output
+ * (reached from `self.vae.encode(image).latent_dist` in the i2vgen pipeline :496 and the svd pipeline :221), then the
+ * layouts the two denoising loops take.  Run once per call, not per step.
+ * moments: channels-last bf16 [n, hw, 8] = (mean[4], logvar[4]); noise: DEVICE fp32 [n, 4, hw] or NULL (no noise).
+ *   v = mean + exp(0.5 * clamp(logvar, -30, 20)) * noise       (v = mean when noise is NULL; fp32, one rounding)
+ * layout / out (bf16):
+ *   CA_VAE_POSTERIOR  [n, 4, hw]             v  (latent_dist.sample() / .mode()); frames = num_videos = 1
+ *   CA_VAE_I2VGEN     [2*n*nv, 4, frames, hw] frame 0 = v * scale, frame k >= 1 = k / (frames - 1); the n images tiled
+ *                                            nv times, then twice for classifier-free guidance (i2vgen pipeline :487-517)
+ *   CA_VAE_SVD        [2*n*nv, frames, 4, hw] cat([zeros, v]) repeated nv times, then repeated over the frames
+ *                                            (svd pipeline :214-235, :580-583)
+ * latent_channels must be 4.
+ */
+enum ca_vae_layout { CA_VAE_POSTERIOR = 0, CA_VAE_I2VGEN = 1, CA_VAE_SVD = 2 };
+int ca_vae_latents(const void* moments, const float* noise, int32_t n, int64_t hw, int32_t latent_channels,
+                   int32_t layout, int32_t frames, int32_t num_videos, float scale, void* out, void* cuda_stream);
+
+/*
  * Temporal self-attention over the frame axis (diffusers TemporalBasicTransformerBlock.attn1 reached from
  * model/adapter_spatial_temporal.py:280).  q/k/v: rows of heads*64 bf16 with stride in_row_stride elements (views of a
  * fused QKV buffer), out: [clips*frames*hw, heads*64] dense; rows in (clip, frame, pixel)
