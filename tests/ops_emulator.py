@@ -78,14 +78,21 @@ def _unpack_conv_weight(w_packed, ntaps, kpt, cin):
 
 
 def conv2d(x, w_packed, bias, *, ksize=3, stride=1, x2=None, act=ACT_NONE, out_scale=1.0, rowvec=None, residual=None,
-           blend_src=None, blend_alpha=None, out=None, out_fp32=False, bn=0, k_per_tap=None):
+           blend_src=None, blend_alpha=None, out=None, out_fp32=False, bn=0, k_per_tap=None, pad=None):
+    """pad (0, 1) at stride 2: one zero row / column at the bottom / right, then an unpadded convolution"""
     n, h, w_, c = x.shape
     xin = x if x2 is None else torch.cat([x, x2], dim=3)
     cin = xin.shape[3]
     ntaps = ksize * ksize
     kpt = k_per_tap if k_per_tap is not None else w_packed.shape[1] // ntaps
     wt = _unpack_conv_weight(w_packed, ntaps, kpt, cin).permute(0, 2, 1).reshape(-1, cin, ksize, ksize)
-    acc = F.conv2d(xin.float().permute(0, 3, 1, 2), wt, None, stride=stride, padding=ksize // 2).permute(0, 2, 3, 1)
+    xf = xin.float().permute(0, 3, 1, 2)
+    if pad is None or tuple(pad) == (ksize // 2,) * 2:
+        acc = F.conv2d(xf, wt, None, stride=stride, padding=ksize // 2)
+    else:
+        assert tuple(pad) == (0, 1) and stride == 2, pad
+        acc = F.conv2d(F.pad(xf, (0, 1, 0, 1)), wt, None, stride=2)
+    acc = acc.permute(0, 2, 3, 1)
     rv = None
     if rowvec is not None:
         rv = rowvec.reshape(rowvec.shape[0], 1, 1, -1)
@@ -336,9 +343,27 @@ def cfg_ddim(eps_uncond, eps_text, latents, guidance, step_row, latents_out=None
     return latents_out
 
 
+def vae_latents(moments, layout=0, noise=None, frames=1, num_videos=1, scale=1.0):
+    """ca_vae_latents: posterior of the quant_conv output (mean, logvar in channels 0-3 / 4-7), then the image-latent
+    layout of the posterior (0), the I2VGen-XL loop (1) or the SVD loop (2); fp32 arithmetic, one rounding to bf16."""
+    m = moments.float().permute(0, 3, 1, 2)
+    v = m[:, :4]
+    if noise is not None:
+        v = v + torch.exp(0.5 * m[:, 4:].clamp(-30.0, 20.0)) * noise.float()
+    if layout == 0:
+        return v.to(BF16)
+    if layout == 1:
+        pos = [torch.full_like(v[:, :, None], k / (frames - 1)) for k in range(1, frames)]
+        x = torch.cat([(v * scale)[:, :, None]] + pos, dim=2).repeat(num_videos, 1, 1, 1, 1)
+        return torch.cat([x, x]).to(BF16)
+    x = torch.cat([torch.zeros_like(v), v]).repeat(num_videos, 1, 1, 1)
+    return x[:, None].repeat(1, frames, 1, 1, 1).to(BF16)
+
+
 _EMULATED = ["linear", "conv2d", "temporal_conv", "attention", "temporal_attention", "group_norm", "layer_norm",
              "timestep_embedding", "silu", "add", "nchw_to_nhwc", "nhwc_to_nchw", "avgpool", "upsample2x", "i2vgen_latent_encoder",
-             "softmax_rows", "frame_conv_small", "router_weights", "router_merge", "cfg_euler", "cfg_euler_v", "cfg_ddim"]
+             "softmax_rows", "frame_conv_small", "router_weights", "router_merge", "cfg_euler", "cfg_euler_v", "cfg_ddim",
+             "vae_latents"]
 
 
 @contextlib.contextmanager

@@ -64,47 +64,28 @@ def test_conv2d_pad_bottom_right(c, h, w):
     assert float((sym - ref).abs().max()) > 10 * err  # the two paddings are far apart on this input
 
 
-def _ulp_bf16(v: torch.Tensor) -> torch.Tensor:
-    a = v.abs().clamp_min(2.0 ** -126)
-    return torch.exp2(torch.floor(torch.log2(a)) - 7)
-
-
 @pytest.mark.parametrize("frames", [1, 2, 16])
 @pytest.mark.parametrize("nv", [1, 2])
 def test_vae_latents_kernel(frames, nv):
-    """ca_vae_latents vs a float64 statement: zeros, position planes and mode bit-exact, sample within one bf16 ulp"""
+    """ca_vae_latents vs the float64 statement of kernel_checks.vae_latents_verdict: zeros, position planes and mode
+    bit-exact, sample within one bf16 ulp"""
     from ctrl_adapter_b200 import ops
+    from tests import kernel_checks as kc
     g = torch.Generator().manual_seed(frames * 10 + nv)
     n, h, w = 2, 12, 20
     mom = torch.randn(n, h, w, 8, generator=g)
     mom[..., 4:] = mom[..., 4:] * 12.0  # logvar beyond both clamp bounds somewhere
-    mom = mom.to(BF16)
-    noise = torch.randn(n, 4, h, w, generator=g)
-    scale = 0.18215
-    m64 = mom.double().permute(0, 3, 1, 2)
-    mean, logvar = m64[:, :4], m64[:, 4:].clamp(-30, 20)
-    smp64 = mean + torch.exp(0.5 * logvar) * noise.double()
-    mc, nc = mom.cuda(), noise.cuda()
-    mode = ops.vae_latents(mc).cpu()
-    smp = ops.vae_latents(mc, noise=nc).cpu()
-    i2v = ops.vae_latents(mc, ops.VAE_I2VGEN, nc, frames, nv, scale).cpu()
-    svd = ops.vae_latents(mc, ops.VAE_SVD, None, frames, nv).cpu()
-    torch.cuda.synchronize()
-    assert torch.equal(mode, mean.to(BF16))
-    assert bool(((smp.double() - smp64).abs() <= _ulp_bf16(smp64)).all())
-    # I2VGen-XL: rows r -> image r % n; frame 0 = sample * scale, frame k = k / (F - 1)
-    assert i2v.shape == (2 * n * nv, 4, frames, h, w)
-    for r in range(2 * n * nv):
-        f0 = smp64[r % n] * scale
-        assert bool(((i2v[r, :, 0].double() - f0).abs() <= _ulp_bf16(f0)).all())
-        for k in range(1, frames):
-            assert bool((i2v[r, :, k] == torch.tensor(k / (frames - 1), dtype=torch.float64).to(BF16)).all())
-    # SVD: [zeros, mode] repeated nv times, every frame
-    assert svd.shape == (2 * n * nv, frames, 4, h, w)
-    for r in range(2 * n * nv):
-        q = r % (2 * n)
-        want = torch.zeros(4, h, w, dtype=BF16) if q < n else mean[q - n].to(BF16)
-        assert all(torch.equal(svd[r, f], want) for f in range(frames))
+    mc, nc = mom.to(BF16).cuda(), torch.randn(n, 4, h, w, generator=g).cuda()
+    calls = [(ops.VAE_POSTERIOR, None), (ops.VAE_POSTERIOR, nc), (ops.VAE_I2VGEN, nc), (ops.VAE_SVD, None)]
+    shapes = [(n, 4, h, w), (n, 4, h, w), (2 * n * nv, 4, frames, h, w), (2 * n * nv, frames, 4, h, w)]
+    for (layout, noise), shape in zip(calls, shapes):
+        f, v = (1, 1) if layout == ops.VAE_POSTERIOR else (frames, nv)
+        a = dict(moments=mc, layout=layout, noise=noise, frames=f, num_videos=v, scale=0.18215)
+        out = ops.vae_latents(**a)
+        torch.cuda.synchronize()
+        assert out.shape == shape
+        rec = kc.vae_latents_verdict(f"vae_latents layout {layout} noise {noise is not None}", a, out)
+        assert rec["ok"], rec
 
 
 # ---- pipelines ------------------------------------------------------------------------------------------------------

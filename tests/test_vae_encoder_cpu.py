@@ -2,14 +2,12 @@
 preprocessing of the two video pipelines: module wiring over the emulated op layer vs the restated diffusers encoder,
 key sets and parameter counts, the loading rules, ``ca_vae_latents`` argument checks, and the preprocessing
 restatements (no GPU needed)."""
-import contextlib
 import json
 import os
 
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle.weights import seeded_init_, seeded_tensor
 from tests import ops_emulator as emu
@@ -21,51 +19,6 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref
 
 def _q(t):
     return t.to(BF16).float()
-
-
-def _conv2d_padded(x, w_packed, bias, *, pad=None, **kw):
-    """ops.conv2d with its `pad` argument: (0, 1) at stride 2 is F.pad(x, (0, 1, 0, 1)) and an unpadded convolution;
-    everything else is the emulator's symmetric convolution."""
-    if pad is None or tuple(pad) == (kw.get("ksize", 3) // 2,) * 2:
-        return emu.conv2d(x, w_packed, bias, **kw)
-    assert tuple(pad) == (0, 1) and kw.get("stride") == 2 and kw.get("x2") is None
-    ksize = kw.get("ksize", 3)
-    cin = x.shape[3]
-    wt = emu._unpack_conv_weight(w_packed, ksize * ksize, w_packed.shape[1] // (ksize * ksize), cin)
-    wt = wt.permute(0, 2, 1).reshape(-1, cin, ksize, ksize)
-    xin = F.pad(x.float().permute(0, 3, 1, 2), (0, 1, 0, 1))
-    acc = F.conv2d(xin, wt, None, stride=2).permute(0, 2, 3, 1)
-    return emu._epilogue(acc, bias, kw.get("act", 0), kw.get("out_scale", 1.0), None, kw.get("residual"), None, None,
-                         kw.get("out_fp32", False)).contiguous()
-
-
-def _vae_latents(moments, layout=0, noise=None, frames=1, num_videos=1, scale=1.0):
-    """ca_vae_latents: posterior of the quant_conv output (mean, logvar in channels 0-3 / 4-7), then the image-latent
-    layout of the posterior (0), the I2VGen-XL loop (1) or the SVD loop (2); fp32 arithmetic, one rounding to bf16."""
-    m = moments.float().permute(0, 3, 1, 2)
-    v = m[:, :4]
-    if noise is not None:
-        v = v + torch.exp(0.5 * m[:, 4:].clamp(-30.0, 20.0)) * noise.float()
-    if layout == 0:
-        return v.to(BF16)
-    if layout == 1:
-        pos = [torch.full_like(v[:, :, None], k / (frames - 1)) for k in range(1, frames)]
-        x = torch.cat([(v * scale)[:, :, None]] + pos, dim=2).repeat(num_videos, 1, 1, 1, 1)
-        return torch.cat([x, x]).to(BF16)
-    x = torch.cat([torch.zeros_like(v), v]).repeat(num_videos, 1, 1, 1)
-    return x[:, None].repeat(1, frames, 1, 1, 1).to(BF16)
-
-
-@contextlib.contextmanager
-def _patched():
-    """the emulated op layer plus the two entry points the encoder adds: conv2d's `pad` and vae_latents"""
-    with emu.patched_ops() as ops:
-        saved = ops.conv2d, ops.vae_latents
-        ops.conv2d, ops.vae_latents = _conv2d_padded, _vae_latents
-        try:
-            yield ops
-        finally:
-            ops.conv2d, ops.vae_latents = saved
 
 
 def _image(n, h, w, seed_name="enc_x"):
@@ -99,7 +52,7 @@ def test_emulated_encode_matches_oracle(temporal):
     o, m = _pair(temporal, 21 if temporal else 20)
     x = _image(2, 64, 96)
     noise = seeded_tensor("enc_noise", (2, 4, 8, 12))
-    with torch.no_grad(), _patched():
+    with torch.no_grad(), emu.patched_ops():
         post_ref = o.encode(x)[0]
         post = m.encode(x).latent_dist
         mode, smp = post.mode(), post.sample(noise=noise)
@@ -148,7 +101,7 @@ def test_loading_rules():
     o, m = _pair(False, 20)
     x = _image(1, 32, 32)
     z = _q(seeded_tensor("vae_z", (1, 4, 4, 4)))
-    with torch.no_grad(), _patched():
+    with torch.no_grad(), emu.patched_ops():
         assert m.encoder_loaded and m.encode(x).latent_dist.mode().shape == (1, 4, 4, 4)
         ref_dec = m.decode(z).sample
     dec_only = seeded_init_(odec.AutoencoderKL(**KW), 20).state_dict()
@@ -156,7 +109,7 @@ def test_loading_rules():
     m2.load_state_dict(dec_only)
     assert not m2.encoder_loaded
     m2 = m2.to(BF16).eval()
-    with torch.no_grad(), _patched():
+    with torch.no_grad(), emu.patched_ops():
         with pytest.raises(ValueError, match="encoder weights were not loaded"):
             m2.encode(x)
         assert torch.equal(m2.decode(z).sample, ref_dec)
@@ -166,7 +119,7 @@ def test_loading_rules():
     m3.load_state_dict(sd)
     assert not m3.encoder_loaded
     m3 = m3.to(BF16).eval()
-    with torch.no_grad(), _patched():
+    with torch.no_grad(), emu.patched_ops():
         assert torch.equal(m3.decode(z).sample, ref_dec)
     with pytest.raises(RuntimeError, match="missing keys"):
         AutoencoderKL(**KW).load_state_dict({k: v for k, v in dec_only.items() if k != "post_quant_conv.bias"})
@@ -205,10 +158,10 @@ def test_vae_latents_emulation_layouts():
     mean, logvar = mom.float().permute(0, 3, 1, 2).chunk(2, dim=1)
     smp = mean + torch.exp(0.5 * logvar.clamp(-30, 20)) * noise
     for f, nv in ((1, 1), (3, 2), (16, 1)):
-        a = _vae_latents(mom, 1, noise, f, nv, 0.18215)
+        a = emu.vae_latents(mom, 1, noise, f, nv, 0.18215)
         b = i2vgen_prepare_image_latents(smp * 0.18215, f, nv).to(BF16)
         assert a.shape == (2 * n * nv, 4, f, h, w) and torch.equal(a, b)
-        a = _vae_latents(mom, 2, None, f, nv)
+        a = emu.vae_latents(mom, 2, None, f, nv)
         b = svd_image_latents(mean, f, nv).to(BF16)
         assert a.shape == (2 * n * nv, f, 4, h, w) and torch.equal(a, b)
 
