@@ -20,53 +20,8 @@ from torch import nn
 from . import ops
 from .persistence import PretrainedMixin
 from .layers import (BF16, BasicTransformerBlock, FeedForward, Attention, Linear, Norm, Packable, ResnetBlock2D,
-                     TemporalConv, TimestepEmbedding)
+                     TemporalConv, TimestepEmbedding, _ConfigDict, as_nchw, shared_timestep, to_channels_last_bf16)
 from .ops import ACT_NONE
-
-
-# ------------------------------------------------------------------------------------------------
-# boundary helpers
-# ------------------------------------------------------------------------------------------------
-def to_channels_last_bf16(x: torch.Tensor, c_pad: Optional[int] = None) -> torch.Tensor:
-    """logical NCHW (any memory format, bf16/fp32) -> physical [N, H, W, C] bf16 contiguous."""
-    n, c, h, w = x.shape
-    cp = c if c_pad is None else c_pad
-    if x.dtype == BF16 and cp == c and x.permute(0, 2, 3, 1).is_contiguous():
-        return x.permute(0, 2, 3, 1)
-    if not x.is_contiguous():
-        x = x.contiguous()
-    if x.dtype not in (BF16, torch.float32):
-        x = x.float()
-    return ops.nchw_to_nhwc(x, cp)
-
-
-def as_nchw(y: torch.Tensor) -> torch.Tensor:
-    """physical NHWC -> logical NCHW view (channels_last memory format, no copy)."""
-    return y.permute(0, 3, 1, 2)
-
-
-def timestep_vector(timestep, n: int, device) -> torch.Tensor:
-    """The forms accepted by adapter_spatial_temporal.py:190-198 -> fp32 device vector of length n.
-    A device tensor is consumed without a host sync (the reference's torch.Tensor([t]) forces one, quirk Q17)."""
-    if isinstance(timestep, (int, float)):
-        return torch.full((n,), float(timestep), device=device, dtype=torch.float32)
-    if not isinstance(timestep, torch.Tensor):
-        raise TypeError(f"unsupported timestep type {type(timestep)}")
-    t = timestep.to(device=device, dtype=torch.float32)
-    if t.dim() == 0 or t.numel() == 1:
-        return t.reshape(1).expand(n).contiguous()
-    if t.dim() == 2:
-        t = t.squeeze()
-    return t.reshape(-1).contiguous()
-
-
-def shared_timestep(timestep, device) -> torch.Tensor:
-    """The step's ONE timestep as a [1] fp32 device tensor.  Every kernel path here shares a single timestep across the
-    batch (the pipelines pass a 0-dim `t`); a tensor with several entries would be silently truncated, so it is refused
-    instead (checking that the entries are equal would cost a host sync per call)."""
-    if isinstance(timestep, torch.Tensor) and timestep.numel() > 1:
-        raise NotImplementedError("per-sample timesteps: pass the step's single timestep (0-dim / 1-element / number)")
-    return timestep_vector(timestep, 1, device)[:1].contiguous()
 
 
 class AlphaBlender(Packable):
@@ -273,10 +228,6 @@ def _prep_ctx(ehs: torch.Tensor) -> torch.Tensor:
     return ehs.to(BF16).contiguous()
 
 
-class _ConfigDict(dict):
-    __getattr__ = dict.__getitem__
-
-
 class ControlNetAdapter(PretrainedMixin, nn.Module):
     """ctrl_adapter.py:12-224 (num_repeats == 1)."""
 
@@ -315,14 +266,6 @@ class ControlNetAdapter(PretrainedMixin, nn.Module):
         self.down_blocks_adapter = nn.ModuleList([AdapterSpatioTemporal(in_channels=c, out_channels=c, **kw) for c in chans])
         self.mid_block_adapter = AdapterSpatioTemporal(in_channels=1280, out_channels=1280, **kw) \
             if add_adapter_location_M else None
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
 
     def get_down_block_ids(self):
         ids = []
@@ -419,10 +362,6 @@ class ControlNetRouter(PretrainedMixin, nn.Module):
         if add_mid_block_router:
             self.mid_block_router = cls(num_experts)
         self.register_buffer("_anchor", torch.zeros(1), persistent=False)
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
 
     def _logits(self) -> torch.Tensor:
         mods = list(self.down_blocks_router) + ([self.mid_block_router] if self.add_mid_block_router else [])

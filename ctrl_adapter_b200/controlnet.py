@@ -13,8 +13,8 @@ from torch import nn
 
 from . import ops
 from .persistence import PretrainedMixin
-from .adapter import _ConfigDict, as_nchw, shared_timestep, to_channels_last_bf16
-from .layers import BF16, Conv2d, ResnetBlock2D, TimestepEmbedding, Transformer2DModel
+from .layers import (BF16, Conv2d, DownBlock2D, MidBlock2D, ResnetBlock2D, TimestepEmbedding, Transformer2DModel,
+                     _ConfigDict, as_nchw, shared_timestep, to_channels_last_bf16)
 from .ops import ACT_SILU
 
 
@@ -41,43 +41,14 @@ class ControlNetConditioningEmbedding(nn.Module):
         return self.conv_out(e)
 
 
-class _DownBlock(nn.Module):
-    def __init__(self, cin, cout, temb, eps, heads, cross_dim, has_attn, add_downsample, layers=2):
-        super().__init__()
-        self.has_cross_attention = has_attn
-        self.resnets = nn.ModuleList([ResnetBlock2D(cin if i == 0 else cout, cout, temb, eps) for i in range(layers)])
-        if has_attn:
-            self.attentions = nn.ModuleList([Transformer2DModel(heads, cout // heads, cout, 1, cross_dim, False)
-                                             for _ in range(layers)])
-        self.downsamplers = None
-        if add_downsample:
-            ds = nn.Module()
-            ds.conv = Conv2d(cout, cout, 3, stride=2)
-            self.downsamplers = nn.ModuleList([ds])
-
-    def forward(self, x, temb_act, ctx):
-        outs = []
-        for i, r in enumerate(self.resnets):
-            x = r(x, temb_act)
-            if self.has_cross_attention:
-                x = self.attentions[i](x, ctx)
-            outs.append(x)
-        if self.downsamplers is not None:
-            x = self.downsamplers[0].conv(x)
-            outs.append(x)
-        return x, outs
+def _attentions(n, heads, c, cross_dim):
+    return [Transformer2DModel(heads, c // heads, c, 1, cross_dim, False) for _ in range(n)]
 
 
-class _MidBlock(nn.Module):
-    def __init__(self, c, temb, eps, heads, cross_dim):
-        super().__init__()
-        self.resnets = nn.ModuleList([ResnetBlock2D(c, c, temb, eps), ResnetBlock2D(c, c, temb, eps)])
-        self.attentions = nn.ModuleList([Transformer2DModel(heads, c // heads, c, 1, cross_dim, False)])
-
-    def forward(self, x, temb_act, ctx):
-        x = self.resnets[0](x, temb_act)
-        x = self.attentions[0](x, ctx)
-        return self.resnets[1](x, temb_act)
+def _down(cin, cout, temb, eps, heads, cross_dim, has_attn, add_downsample):
+    return DownBlock2D([ResnetBlock2D(cin if i == 0 else cout, cout, temb, eps) for i in range(2)],
+                       _attentions(2, heads, cout, cross_dim) if has_attn else None,
+                       Conv2d(cout, cout, 3, stride=2) if add_downsample else None)
 
 
 class ControlNetModel(PretrainedMixin, nn.Module):
@@ -128,23 +99,17 @@ class ControlNetModel(PretrainedMixin, nn.Module):
         for i, t in enumerate(down_block_types):
             in_c, out_c = out_c, block_out_channels[i]
             final = i == len(block_out_channels) - 1
-            self.down_blocks.append(_DownBlock(in_c, out_c, temb, norm_eps, heads, cross_attention_dim,
-                                               t == "CrossAttnDownBlock2D", not final))
+            self.down_blocks.append(_down(in_c, out_c, temb, norm_eps, heads, cross_attention_dim,
+                                          t == "CrossAttnDownBlock2D", not final))
             for _ in range(layers_per_block + (0 if final else 1)):
                 self.controlnet_down_blocks.append(Conv2d(out_c, out_c, 1))
         self.controlnet_mid_block = Conv2d(block_out_channels[-1], block_out_channels[-1], 1)
         if mid_block_type != "UNetMidBlock2DCrossAttn":
             raise NotImplementedError(mid_block_type)
-        self.mid_block = _MidBlock(block_out_channels[-1], temb, norm_eps, heads, cross_attention_dim)
+        c = block_out_channels[-1]
+        self.mid_block = MidBlock2D([ResnetBlock2D(c, c, temb, norm_eps), ResnetBlock2D(c, c, temb, norm_eps)],
+                                    _attentions(1, heads, c, cross_attention_dim))
         self._static_cond = None
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
 
     @torch.no_grad()
     def cache_static_cond(self, controlnet_cond: torch.Tensor):

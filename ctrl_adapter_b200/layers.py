@@ -5,8 +5,9 @@ Each class is an ``nn.Module`` used ONLY as a parameter container with the refer
 launches the sm_90a kernels of ``csrc/`` through ``ops``.  Activations are channels-last bf16.
 
 Weights are repacked once (``pack()``, lazily on first use / after ``.to()``) into the kernel layouts:
-conv weights ``[Cout, taps*Cin]``, fused QKV / KV projection matrices, GEGLU rows interleaved per 256-wide N tile,
-head dims zero-padded to multiples of 64 (SD1.5 ControlNet heads are 40/80/160 wide), biases as fp32.
+conv weights ``[Cout, taps*Cin]`` (Cout and Cin zero padded to multiples of 8), fused QKV / KV projection matrices,
+GEGLU rows interleaved per 256-wide N tile, head dims zero-padded to multiples of 64 (SD1.5 ControlNet heads are
+40/80/160 wide), biases as fp32.
 """
 from __future__ import annotations
 
@@ -22,6 +23,55 @@ from .ops import ACT_GEGLU, ACT_NONE, ACT_SILU, BF16
 
 def _pad64(d: int) -> int:
     return (d + 63) // 64 * 64
+
+
+# ------------------------------------------------------------------------------------------------
+# boundary helpers
+# ------------------------------------------------------------------------------------------------
+def to_channels_last_bf16(x: torch.Tensor, c_pad: Optional[int] = None) -> torch.Tensor:
+    """logical NCHW (any memory format, bf16/fp32) -> physical [N, H, W, C] bf16 contiguous."""
+    n, c, h, w = x.shape
+    cp = c if c_pad is None else c_pad
+    if x.dtype == BF16 and cp == c and x.permute(0, 2, 3, 1).is_contiguous():
+        return x.permute(0, 2, 3, 1)
+    if not x.is_contiguous():
+        x = x.contiguous()
+    if x.dtype not in (BF16, torch.float32):
+        x = x.float()
+    return ops.nchw_to_nhwc(x, cp)
+
+
+def as_nchw(y: torch.Tensor) -> torch.Tensor:
+    """physical NHWC -> logical NCHW view (channels_last memory format, no copy)."""
+    return y.permute(0, 3, 1, 2)
+
+
+def timestep_vector(timestep, n: int, device) -> torch.Tensor:
+    """The forms accepted by adapter_spatial_temporal.py:190-198 -> fp32 device vector of length n.
+    A device tensor is consumed without a host sync (the reference's torch.Tensor([t]) forces one, quirk Q17)."""
+    if isinstance(timestep, (int, float)):
+        return torch.full((n,), float(timestep), device=device, dtype=torch.float32)
+    if not isinstance(timestep, torch.Tensor):
+        raise TypeError(f"unsupported timestep type {type(timestep)}")
+    t = timestep.to(device=device, dtype=torch.float32)
+    if t.dim() == 0 or t.numel() == 1:
+        return t.reshape(1).expand(n).contiguous()
+    if t.dim() == 2:
+        t = t.squeeze()
+    return t.reshape(-1).contiguous()
+
+
+def shared_timestep(timestep, device) -> torch.Tensor:
+    """The step's ONE timestep as a [1] fp32 device tensor.  Every kernel path here shares a single timestep across the
+    batch (the pipelines pass a 0-dim `t`); a tensor with several entries would be silently truncated, so it is refused
+    instead (checking that the entries are equal would cost a host sync per call)."""
+    if isinstance(timestep, torch.Tensor) and timestep.numel() > 1:
+        raise NotImplementedError("per-sample timesteps: pass the step's single timestep (0-dim / 1-element / number)")
+    return timestep_vector(timestep, 1, device)[:1].contiguous()
+
+
+class _ConfigDict(dict):
+    __getattr__ = dict.__getitem__
 
 
 class Packable(nn.Module):
@@ -88,12 +138,21 @@ class Conv2d(Packable):
         nn.init.normal_(self.weight, std=1.0 / math.sqrt(i * k * k))
 
     def pack(self):
+        """-> weight [ceil8(Cout), taps * Kp] bf16, bias [ceil8(Cout)] fp32.  Cin is zero padded to a multiple of 8
+        (e.g. 4 latent / 3 image channels: the activations are zero padded to 8).  Cout is zero padded the same way (zero
+        weight rows, zero bias) because the kernel stores 16-byte vectors: the output then has ceil8(Cout) channels, of
+        which the first Cout are real and the rest are zeros (e.g. a UNet's 4-channel conv_out writes [N, H, W, 8])."""
         cin_eff = (self.cin + 7) // 8 * 8
+        cout_eff = (self.cout + 7) // 8 * 8
         kpad = 64 if self.stride == 2 else 8
         w = self.weight.detach()
-        if cin_eff != self.cin:  # e.g. 4 latent / 3 image channels: activations are zero padded to 8
+        b = _f32(self.bias)
+        if cin_eff != self.cin:
             w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cin_eff - self.cin))
-        return ops.pack_conv_weight(w, kpad), _f32(self.bias)
+        if cout_eff != self.cout:
+            w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, 0, 0, cout_eff - self.cout))
+            b = torch.nn.functional.pad(b, (0, cout_eff - self.cout))
+        return ops.pack_conv_weight(w, kpad), b
 
     def forward(self, x, x2=None, **kw):
         w, b = self.packed()
@@ -406,3 +465,91 @@ class Transformer2DModel(nn.Module):
         w, b = self._w(self.proj_out)
         out = ops.linear(h.reshape(n * hh * ww, -1), w, b, residual=x.reshape(n * hh * ww, c))
         return out.reshape(n, hh, ww, c)
+
+
+# ------------------------------------------------------------------------------------------------
+# diffusers' 2-D UNet block wiring, shared by the SDXL UNet, the SVD UNet and the ControlNet.  The blocks take their
+# already-built resnets / attentions: ResnetBlock2D + Transformer2DModel, or SpatioTemporalResBlock +
+# TransformerSpatioTemporalModel, whose forward()s take a trailing `frames` argument -- passed through as *frames.
+# ------------------------------------------------------------------------------------------------
+def _sampler(conv: Conv2d) -> nn.ModuleList:
+    """Downsample2D / Upsample2D container (state-dict keys downsamplers.0.conv.* / upsamplers.0.conv.*)."""
+    s = nn.Module()
+    s.conv = conv
+    return nn.ModuleList([s])
+
+
+class DownBlock2D(nn.Module):
+    """(CrossAttn)DownBlock2D: resnet [-> attention] per layer, then the optional stride-2 conv; every layer's output
+    and the down-sampled one are skips."""
+
+    def __init__(self, resnets, attentions=None, downsampler: Optional[Conv2d] = None):
+        super().__init__()
+        self.has_cross_attention = attentions is not None
+        self.resnets = nn.ModuleList(resnets)
+        if attentions is not None:
+            self.attentions = nn.ModuleList(attentions)
+        self.downsamplers = None if downsampler is None else _sampler(downsampler)
+
+    def forward(self, x, temb_act, ctx, *frames):
+        outs = []
+        for i, r in enumerate(self.resnets):
+            x = r(x, temb_act, *frames)
+            if self.has_cross_attention:
+                x = self.attentions[i](x, ctx, *frames)
+            outs.append(x)
+        if self.downsamplers is not None:
+            x = self.downsamplers[0].conv(x)
+            outs.append(x)
+        return x, outs
+
+
+class MidBlock2D(nn.Module):
+    """UNetMidBlock2DCrossAttn: resnet, then (attention, resnet) per attention."""
+
+    def __init__(self, resnets, attentions):
+        super().__init__()
+        self.resnets = nn.ModuleList(resnets)
+        self.attentions = nn.ModuleList(attentions)
+
+    def forward(self, x, temb_act, ctx, *frames):
+        x = self.resnets[0](x, temb_act, *frames)
+        for attn, r in zip(self.attentions, self.resnets[1:]):
+            x = r(attn(x, ctx, *frames), temb_act, *frames)
+        return x
+
+
+class UpBlock2D(nn.Module):
+    """(CrossAttn)UpBlock2D: per layer, resnet on (x, the last skip) [-> attention]; then the optional 2x nearest
+    up-sampling + conv.  The skip is the resnet's second input source, never concatenated in memory."""
+
+    def __init__(self, resnets, attentions=None, upsampler: Optional[Conv2d] = None):
+        super().__init__()
+        self.has_cross_attention = attentions is not None
+        self.resnets = nn.ModuleList(resnets)
+        if attentions is not None:
+            self.attentions = nn.ModuleList(attentions)
+        self.upsamplers = None if upsampler is None else _sampler(upsampler)
+
+    def forward(self, x, temb_act, ctx, *frames, skips):
+        for i, r in enumerate(self.resnets):
+            x = r(x, temb_act, *frames, x2=skips.pop())
+            if self.has_cross_attention:
+                x = self.attentions[i](x, ctx, *frames)
+        if self.upsamplers is not None:
+            x = self.upsamplers[0].conv(ops.upsample2x(x))
+        return x
+
+
+def add_residual(x, r: torch.Tensor):
+    """x [B*F, H, W, C] + an adapter / ControlNet residual given as logical NCHW, 4-D "(b f) c h w" or 5-D "b c f h w"
+    (any memory format)."""
+    if r.dim() == 5:
+        r = r.permute(0, 2, 1, 3, 4).flatten(0, 1)
+    return ops.add(x, to_channels_last_bf16(r))
+
+
+def add_skip_residuals(skips: list, residuals):
+    """skips[i] = add_residual(skips[i], residuals[i]), truncated to the shorter list as the reference's zip() does."""
+    for i, (s, r) in enumerate(zip(skips, residuals)):
+        skips[i] = add_residual(s, r)

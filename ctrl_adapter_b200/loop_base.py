@@ -1,4 +1,5 @@
-"""What the three denoising loops share: the per-step control schedule (``controlnet_keep``), eager / CUDA-graph stepping.
+"""What the three denoising loops share: the per-step control schedule (``controlnet_keep``), the pooling of the control
+path to the ControlNet's 512x512 / 64x64 geometry, the video loops' key-frame adapter path, eager / CUDA-graph stepping.
 
 Reference: the ``controlnet_keep`` list and ``cond_scale = controlnet_conditioning_scale * controlnet_keep[i]`` of
 /root/reference/sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:1207-1211, :1296-1302 (identical code in
@@ -14,6 +15,9 @@ from typing import Dict, List, Optional, Sequence, Union
 
 import torch
 
+from . import ops
+from .layers import BF16, as_nchw, to_channels_last_bf16
+
 Scale = Union[float, tuple]
 
 
@@ -21,6 +25,23 @@ def controlnet_keep(num_steps: int, start: Sequence[float], end: Sequence[float]
     """keeps[i][k] for ControlNet k at step i -- the reference's list comprehension, verbatim semantics."""
     return [[1.0 - float(i / num_steps < s or (i + 1) / num_steps > e) for s, e in zip(start, end)]
             for i in range(num_steps)]
+
+
+def pool_control_images(images: torch.Tensor) -> torch.Tensor:
+    """F.adaptive_avg_pool2d(images, (512, 512)) of the loop bodies (sdxl pipeline :1306-1312, svd :664-670).  It does
+    not depend on the step, so the loops run it once in prepare().  images [N, 3, H, W] bf16, H and W multiples of
+    512."""
+    if tuple(images.shape[-2:]) == (512, 512):
+        return images
+    if images.shape[-2] % 512 or images.shape[-1] % 512:
+        raise NotImplementedError("control images must be 512x512 or an integer multiple of it (adaptive pool windows)")
+    return as_nchw(ops.avgpool(to_channels_last_bf16(images, 8), 512, 512))[:, :3].contiguous()
+
+
+def pool_controlnet_input(latents: torch.Tensor) -> torch.Tensor:
+    """F.adaptive_avg_pool2d(latents, (64, 64)): the ControlNet runs at 64x64 latents (512x512) whatever the backbone's
+    resolution (same reference lines).  latents [N, 4, h, w] -> [N, 4, 64, 64], channels-last view."""
+    return as_nchw(ops.avgpool(to_channels_last_bf16(latents, 8), 64, 64))[:, :4]
 
 
 class DenoiseLoopBase:
@@ -42,6 +63,45 @@ class DenoiseLoopBase:
         self._scale = ([float(c) for c in conditioning_scale] if isinstance(conditioning_scale, (list, tuple))
                        else float(conditioning_scale))
         self._graphs: Dict[Scale, torch.cuda.CUDAGraph] = {}
+
+    def _init_key_frames(self, clips: int, frames: int, device):
+        """Rows of the `sparse_frames` key frames in the (clip, frame)-ordered batch of `clips` clips (None: all)."""
+        self._sparse_rows = None
+        if self.sparse_frames is not None:
+            if not all(0 <= k < frames for k in self.sparse_frames):
+                raise ValueError("sparse_frames must index frames of the clip")
+            self._sparse_rows = torch.tensor([c * frames + k for c in range(clips) for k in self.sparse_frames],
+                                             device=device)
+
+    def _video_adapter(self, down, mid, t, n: int, mid_hw):
+        """Ctrl-Adapter of the video loops (i2vgen pipeline :1024-1083, svd :700-750).  down / mid: the ControlNet's
+        residuals for all n frame-samples, or down None when the step's conditioning scale is 0: every ControlNet output
+        is then exactly zero and the down residuals are dropped, but the mid-block adapter's output (a function of t
+        alone, on zeros of spatial size mid_hw) is still injected (quirk Q9).  With sparse_frames, only the key frames
+        go through the adapter (host-side index gather over ControlNet-sized tensors) and are scattered into zero
+        residuals; the reference's dense tensors are fp32 zeros, which only changes where the skip + residual sum is
+        rounded (quirk Q21).  Returns (down residuals or None, mid residual or None)."""
+        rows = self._sparse_rows
+        nf = self.frames if rows is None else len(self.sparse_frames)
+        if down is not None:
+            if rows is not None:
+                down = [d.index_select(0, rows) for d in down]
+                mid = mid.index_select(0, rows) if mid is not None else None
+            down, mid = self.adapter(down, mid_block_res_sample=mid, sparsity_masking=self.sparse_frames,
+                                     num_frames=nf, timestep=t, encoder_hidden_states=self.adapter_ctx)
+        else:
+            mid0 = torch.zeros((n if rows is None else rows.numel(), *mid_hw, 1280), device=t.device,
+                               dtype=BF16).permute(0, 3, 1, 2)
+            mid = self.adapter.forward_mid(mid0, num_frames=nf, timestep=t, encoder_hidden_states=self.adapter_ctx)
+        if rows is None:
+            return down, mid
+
+        def scatter(x):
+            full = torch.zeros((n, *x.shape[1:]), device=x.device, dtype=x.dtype).contiguous(
+                memory_format=torch.channels_last)
+            full.index_copy_(0, rows, x)
+            return full
+        return ([scatter(d) for d in down] if down is not None else None), (scatter(mid) if mid is not None else None)
 
     def control_scale(self, i: int) -> Scale:
         """cond_scale of step i: a float for one ControlNet, a tuple for Multi-ControlNet (reference :1296-1302)."""

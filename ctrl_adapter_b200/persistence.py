@@ -33,10 +33,18 @@ def _jsonable(v):
 
 
 class PretrainedMixin:
-    """``save_pretrained`` / ``from_pretrained`` for an ``nn.Module`` that keeps its constructor arguments in
-    ``self.config`` (a dict)."""
+    """``save_pretrained`` / ``from_pretrained``, and diffusers' ``dtype`` / ``device`` properties, for an ``nn.Module``
+    that keeps its constructor arguments in ``self.config`` (a dict)."""
 
     config_name = CONFIG_NAME
+
+    @property
+    def dtype(self) -> torch.dtype:
+        return next(self.parameters()).dtype
+
+    @property
+    def device(self) -> torch.device:
+        return next(self.parameters()).device
 
     def save_pretrained(self, path: str, safe_serialization: bool = True):
         os.makedirs(path, exist_ok=True)

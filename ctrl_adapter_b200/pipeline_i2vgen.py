@@ -14,8 +14,7 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .adapter import as_nchw, to_channels_last_bf16
-from .layers import cache_static_context
+from .layers import as_nchw, cache_static_context, to_channels_last_bf16
 from .loop_base import DenoiseLoopBase
 from .schedulers import DDIMSchedule
 
@@ -39,10 +38,10 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
         self.sparse_frames = None if sparse_frames is None else [int(k) for k in sparse_frames]
         self.schedule = DDIMSchedule(num_inference_steps)
         self.num_inference_steps = num_inference_steps
-        nets = len(controlnet.nets) if hasattr(controlnet, "nets") else 1
+        multi = hasattr(controlnet, "nets")
         self._init_control(controlnet_conditioning_scale, control_guidance_start, control_guidance_end,
-                           nets if hasattr(controlnet, "nets") else 1)
-        self._multi = hasattr(controlnet, "nets")  # a one-net MultiControlNetModel still takes list arguments
+                           len(controlnet.nets) if multi else 1)
+        self._multi = multi  # a one-net MultiControlNetModel still takes list arguments
 
     def prepare(self, latents, prompt_embeds, image_latents, image_embeddings, fps, controlnet_prompt_embeds,
                 control_images):
@@ -64,22 +63,13 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
         self.image_embeddings = image_embeddings.to(BF16).contiguous()
         self.fps = fps.float().contiguous()
         self.cn_embeds = controlnet_prompt_embeds.to(BF16).contiguous()
-        self._pool = (h, w) != (64, 64) and self.use_size_512                              # :941-947
-        if self._pool:
+        if (h, w) != (64, 64) and self.use_size_512:                                        # :941-947
             # the reference pools the ControlNet input to 64x64 here, but its video adapters do not up-sample, so the
             # 64x64 residuals cannot be added to a UNet running at another size (it fails inside the UNet, :689)
             raise ValueError("use_size_512=True needs 64x64 latents (512x512 video) for the I2VGen-XL backbone; pass "
                              "use_size_512=False to run the ControlNet at the latent resolution")
-
-        def prep_image(img):
-            img = img.to(BF16).contiguous()
-            if self._pool and tuple(img.shape[-2:]) != (512, 512):                         # step-invariant: pooled once
-                if img.shape[-2] % 512 or img.shape[-1] % 512:
-                    raise NotImplementedError("control images must be 512x512 or an integer multiple of it")
-                img = as_nchw(ops.avgpool(to_channels_last_bf16(img, 8), 512, 512))[:, :3].contiguous()
-            return img
-        self.images = ([prep_image(i) for i in control_images] if isinstance(control_images, (list, tuple))
-                       else prep_image(control_images))
+        self.images = ([i.to(BF16).contiguous() for i in control_images] if isinstance(control_images, (list, tuple))
+                       else control_images.to(BF16).contiguous())
         # adapter context: the LAST sample's image embedding for every sample (reference :1048, quirk Q5)
         self.adapter_ctx = self.image_embeddings[-1].unsqueeze(0).contiguous()
         # timestep-independent UNet conditioning, computed once (exact hoist)
@@ -102,11 +92,7 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
             pick = lambda wrow: wrow.repeat_interleave(f)[sel_idx].float().contiguous()  # noqa: E731
             self._router_w = ([pick(dw[k]) for k in range(self.router.num_routers)],
                               pick(mw) if mw is not None else None)
-        self._sparse_rows = None
-        if self.sparse_frames is not None:
-            if not all(0 <= k < f for k in self.sparse_frames):
-                raise ValueError("sparse_frames must index frames of the clip")
-            self._sparse_rows = torch.tensor([bb * f + k for bb in range(2 * b) for k in self.sparse_frames], device=dev)
+        self._init_key_frames(2 * b, f, dev)
         self._graphs = {}
         self.step_index = 0
 
@@ -138,39 +124,10 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
         t = self.row[0:1]
         lat2 = torch.cat([self.model_in, self.model_in], dim=0)                  # (2B, F, 4, h, w) CFG duplication
         n = 2 * b * f
-        rows = self._sparse_rows
-        nf = f if rows is None else len(self.sparse_frames)
-        mask = None if rows is None else self.sparse_frames
-        control_off = (not isinstance(scale, tuple)) and scale == 0              # :1083 (a list never compares == 0)
-        if not control_off:
-            ctrl_in = lat2.reshape(n, *lat2.shape[2:])                           # "(b f) c h w"
-            if self._pool:
-                ctrl_in = as_nchw(ops.avgpool(to_channels_last_bf16(ctrl_in, 8), 64, 64))[:, :4]
-            down, mid = self._controlnet_outputs(ctrl_in, t, scale)
-            if rows is not None:
-                # key-frame gather -> adapter on len(sparse_frames) frames per clip -> scatter into zero residuals
-                # (host-side index glue over ControlNet-sized tensors; the reference's dense tensors are fp32 zeros,
-                # which only changes where the skip + residual sum is rounded -- quirk Q21)
-                down = [d.index_select(0, rows) for d in down]
-                mid = mid.index_select(0, rows) if mid is not None else None
-            down_a, mid_a = self.adapter(down, mid_block_res_sample=mid, sparsity_masking=mask, num_frames=nf,
-                                         timestep=t, encoder_hidden_states=self.adapter_ctx)
-        else:
-            # cond_scale == 0: every ControlNet output is exactly zero and the down residuals are dropped (:1083), but
-            # the mid-block adapter's output (a function of t alone) is still injected (quirk Q9)
-            down_a = None
-            hh, ww = (8, 8) if self._pool else (lat2.shape[-2] // 8, lat2.shape[-1] // 8)
-            rows_n = n if rows is None else rows.numel()
-            mid0 = torch.zeros((rows_n, hh, ww, 1280), device=lat2.device, dtype=BF16).permute(0, 3, 1, 2)
-            mid_a = self.adapter.forward_mid(mid0, num_frames=nf, timestep=t, encoder_hidden_states=self.adapter_ctx)
-        if rows is not None:
-            def densify(x):
-                full = torch.zeros((n, *x.shape[1:]), device=x.device, dtype=x.dtype).contiguous(
-                    memory_format=torch.channels_last)
-                full.index_copy_(0, rows, x)
-                return full
-            down_a = [densify(d) for d in down_a] if down_a is not None else None
-            mid_a = densify(mid_a) if mid_a is not None else None
+        down = mid = None
+        if isinstance(scale, tuple) or scale != 0:                               # :1083 (a list never compares == 0)
+            down, mid = self._controlnet_outputs(lat2.reshape(n, *lat2.shape[2:]), t, scale)  # "(b f) c h w"
+        down_a, mid_a = self._video_adapter(down, mid, t, n, (lat2.shape[-2] // 8, lat2.shape[-1] // 8))
         sample = lat2.permute(0, 2, 1, 3, 4)                                     # (2B, 4, F, h, w) view
         eps = self.unet(sample, t, self.fps, self.image_latents, image_embeddings=self.image_embeddings,
                         encoder_hidden_states=self.prompt_embeds, down_block_additional_residuals=down_a,

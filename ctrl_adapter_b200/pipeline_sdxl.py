@@ -14,9 +14,8 @@ from typing import Optional
 import torch
 
 from . import ops
-from .adapter import as_nchw, to_channels_last_bf16
 from .layers import cache_static_context
-from .loop_base import DenoiseLoopBase
+from .loop_base import DenoiseLoopBase, pool_control_images, pool_controlnet_input
 from .schedulers import EulerDiscreteSchedule
 
 BF16 = torch.bfloat16
@@ -54,13 +53,8 @@ class SDXLControlNetAdapterLoop(DenoiseLoopBase):
                           time_ids=add_time_ids.float().contiguous())
         self.cn_embeds = controlnet_prompt_embeds.to(BF16).contiguous()
         images = control_images.to(BF16).contiguous()
-        h, w = latents.shape[-2:]
-        if (h, w) != (64, 64) and self.use_size_512 and tuple(images.shape[-2:]) != (512, 512):
-            # F.adaptive_avg_pool2d(images, (512, 512)) of the loop body (:1306-1312): step-invariant, done once here
-            if images.shape[-2] % 512 or images.shape[-1] % 512:
-                raise NotImplementedError("control images must be 512x512 or an integer multiple (adaptive pool windows)")
-            images = as_nchw(ops.avgpool(to_channels_last_bf16(images, 8), 512, 512))[:, :3].contiguous()
-        self.images = images
+        self._pool = tuple(latents.shape[-2:]) != (64, 64) and self.use_size_512  # pipeline :1306-1312
+        self.images = pool_control_images(images) if self._pool else images
         # step-invariant work, hoisted (exact: same kernels on the same operands, run once instead of every step):
         # cross-attention K/V of the constant prompt embeddings, the ControlNet's conditioning-image embedding
         cache_static_context(self.unet, self.prompt_embeds)
@@ -85,10 +79,7 @@ class SDXLControlNetAdapterLoop(DenoiseLoopBase):
         if scale != 0:
             # with cond_scale == 0 the reference still runs ControlNet + adapter but discards their output (:1346, and
             # mid_block_additional_residual is the constant 0): skipping the two modules is exact
-            h, w = lat2.shape[-2:]
-            ctrl_in = lat2
-            if (h, w) != (64, 64) and self.use_size_512:  # pipeline :1306-1312
-                ctrl_in = as_nchw(ops.avgpool(to_channels_last_bf16(lat2, 8), 64, 64))[:, :4]
+            ctrl_in = pool_controlnet_input(lat2) if self._pool else lat2
             down, mid = self.controlnet(ctrl_in, t, encoder_hidden_states=self.cn_embeds, controlnet_cond=self.images,
                                         conditioning_scale=scale, guess_mode=False, return_dict=False)
             residuals, _ = self.adapter(down, sparsity_masking=None, num_frames=1, timestep=t,

@@ -17,9 +17,8 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .adapter import as_nchw, to_channels_last_bf16
 from .layers import cache_static_context
-from .loop_base import DenoiseLoopBase
+from .loop_base import DenoiseLoopBase, pool_control_images, pool_controlnet_input
 from .schedulers import EulerKarrasVSchedule
 
 BF16 = torch.bfloat16
@@ -63,21 +62,13 @@ class SVDControlNetAdapterLoop(DenoiseLoopBase):
         images = control_images.to(BF16).contiguous()
         h, w = latents.shape[-2:]
         self._pool = (h, w) != (64, 64) and self.use_size_512                    # :664-670
-        if self._pool and tuple(images.shape[-2:]) != (512, 512):               # step-invariant: pooled once, here
-            if images.shape[-2] % 512 or images.shape[-1] % 512:
-                raise NotImplementedError("control images must be 512x512 or an integer multiple of it")
-            images = as_nchw(ops.avgpool(to_channels_last_bf16(images, 8), 512, 512))[:, :3].contiguous()
-        self.images = images
+        self.images = pool_control_images(images) if self._pool else images
         self.adapter_ctx = self.image_embeddings[-1].unsqueeze(0).contiguous()  # the LAST sample's embedding (:715)
         # step-invariant work, hoisted (exact): single-token contexts, ControlNet text K/V and image embedding
         cache_static_context(self.adapter, self.adapter_ctx, single_token_rows=1)
         cache_static_context(self.controlnet, self.cn_embeds)
         self.controlnet.cache_static_cond(self.images)
-        self._sparse_rows = None
-        if self.sparse_frames is not None:
-            if not all(0 <= k < f for k in self.sparse_frames):
-                raise ValueError("sparse_frames must index frames of the clip")
-            self._sparse_rows = torch.tensor([bb * f + k for bb in range(2 * b) for k in self.sparse_frames], device=dev)
+        self._init_key_frames(2 * b, f, dev)
         self._graphs = {}
         self.step_index = 0
 
@@ -94,43 +85,20 @@ class SVDControlNetAdapterLoop(DenoiseLoopBase):
         lat2 = torch.cat([self.model_in, self.model_in], dim=0)                  # (2B, F, 4, h, w) CFG duplication
         n = 2 * b * f
         h, w = lat2.shape[-2:]
-        rows = self._sparse_rows
-        nf = f if rows is None else len(self.sparse_frames)
-        mask = None if rows is None else self.sparse_frames
-        if scale != 0:
+        down = mid = None
+        if scale != 0:  # cond_scale == 0 (:748): ControlNet outputs are exactly zero, see _video_adapter
             ctrl_in = lat2.reshape(n, 4, h, w)                                   # "b f c h w -> (b f) c h w"
             if self._pool:
-                ctrl_in = as_nchw(ops.avgpool(to_channels_last_bf16(ctrl_in, 8), 64, 64))[:, :4]
+                ctrl_in = pool_controlnet_input(ctrl_in)
             down, mid = self.controlnet(ctrl_in, self.cn_t, encoder_hidden_states=self.cn_embeds,
                                         controlnet_cond=self.images, conditioning_scale=scale, guess_mode=False,
                                         return_dict=False, skip_conv_in=self.skip_conv_in,
                                         skip_time_emb=self.skip_time_emb)
-            if rows is not None:
-                down = [d.index_select(0, rows) for d in down]
-                mid = mid.index_select(0, rows)
-            down_a, mid_a = self.adapter(down, mid_block_res_sample=mid, sparsity_masking=mask, num_frames=nf,
-                                         timestep=self.cn_t, encoder_hidden_states=self.adapter_ctx)
-        else:
-            # cond_scale == 0 (:748): ControlNet outputs are exactly zero, down residuals dropped, mid still injected
-            down_a = None
-            hh, ww = (8, 8) if self._pool else (h // 8, w // 8)
-            mid0 = torch.zeros((n if rows is None else rows.numel(), hh, ww, 1280), device=lat2.device,
-                               dtype=BF16).permute(0, 3, 1, 2)
-            mid_a = self.adapter.forward_mid(mid0, num_frames=nf, timestep=self.cn_t,
-                                             encoder_hidden_states=self.adapter_ctx)
-        if rows is not None:
-            def densify(x):
-                full = torch.zeros((n, *x.shape[1:]), device=x.device, dtype=x.dtype).contiguous(
-                    memory_format=torch.channels_last)
-                full.index_copy_(0, rows, x)
-                return full
-            down_a = [densify(d) for d in down_a] if down_a is not None else None
-            mid_a = densify(mid_a) if mid_a is not None else None
+        down_a, mid_a = self._video_adapter(down, mid, self.cn_t, n, (8, 8) if self._pool else (h // 8, w // 8))
         # the UNet takes "(b f) c h w" residuals as well as the reference's 5-D form; no rearrange needed
-        residuals = down_a
         unet_in = torch.cat([lat2, self.image_latents], dim=2)                   # (2B, F, 8, h, w) channel concat (:755)
         eps = self.unet(unet_in, t, encoder_hidden_states=self.image_embeddings, added_time_ids=self.added_time_ids,
-                        down_block_additional_residuals=residuals, mid_block_additional_residual=mid_a,
+                        down_block_additional_residuals=down_a, mid_block_additional_residual=mid_a,
                         return_dict=False)[0]                                    # (2B, F, 4, h, w)
         ops.cfg_euler_v(eps[:b].contiguous(), eps[b:].contiguous(), self.latents, self.guidance, f, self.row,
                         latents_out=self.latents, model_in_next=self.model_in)

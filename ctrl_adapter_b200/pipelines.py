@@ -109,6 +109,23 @@ class DiffusionPipeline:
     def maybe_free_model_hooks(self):
         pass
 
+    def _controlnet_prompt_embeds(self, prompt, device, embeds, negative_embeds) -> torch.Tensor:
+        """The SD1.5 ControlNet's prompt embeddings, negative half first: passed in, or from the helper's
+        ``encode_controlnet_prompt``."""
+        if embeds is None:
+            helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")
+            embeds, negative_embeds, _, _ = helper.encode_controlnet_prompt(
+                prompt, device, 1, True, negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None,
+                lora_scale=None, clip_skip=None)
+        _need(negative_embeds, "controlnet_negative_prompt_embeds", "SD1.5 prompt helper")
+        return torch.cat([negative_embeds, embeds]).to(device)
+
+    def _denoise(self, loop, num_inference_steps: int, use_cuda_graph: bool):
+        with self.progress_bar(total=num_inference_steps) as bar:
+            for i in range(num_inference_steps):
+                (loop.step_graph if use_cuda_graph else loop.step)(i)
+                bar.update()
+
     @property
     def interrupt(self):
         return self._interrupt
@@ -146,6 +163,21 @@ def _randn(shape, generator, device):
         generator = generator[0]
     gdev = generator.device if generator is not None else torch.device("cpu")
     return torch.randn(shape, generator=generator, device=gdev, dtype=torch.float32).to(device)
+
+
+def _first(v):
+    """the reference's SDXL / SVD loops take one ControlNet: a list argument contributes its first entry"""
+    return v[0] if isinstance(v, list) else v
+
+
+def _per_frame(embeds: torch.Tensor, clips: int, frames: int) -> torch.Tensor:
+    """ControlNet prompt embeddings with one row per clip -> one per frame-sample (i2vgen pipeline :871-874)."""
+    return embeds.repeat_interleave(frames, dim=0) if embeds.shape[0] == clips else embeds
+
+
+def _given_or_encoded(given, encoded):
+    """(image_embeddings, image_latents): the passed tensors keep priority over the ones encode_image built"""
+    return tuple(e if g is None else g for g, e in zip(given, encoded))
 
 
 def _control_tensor(control_images, helper, n, width, height, device):
@@ -371,12 +403,8 @@ class SDXLControlNetAdapterPipeline(DiffusionPipeline):
         _need(negative_prompt_embeds, "negative_prompt_embeds", "text encoder")
         _need(pooled_prompt_embeds, "pooled_prompt_embeds", "text encoder")
         _need(negative_pooled_prompt_embeds, "negative_pooled_prompt_embeds", "text encoder")
-        if controlnet_prompt_embeds is None:
-            helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")
-            controlnet_prompt_embeds, controlnet_negative_prompt_embeds, _, _ = helper.encode_controlnet_prompt(
-                prompt, device, 1, True, negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None,
-                lora_scale=None, clip_skip=None)
-        _need(controlnet_negative_prompt_embeds, "controlnet_negative_prompt_embeds", "SD1.5 prompt helper")
+        cpe = self._controlnet_prompt_embeds(prompt, device, controlnet_prompt_embeds,
+                                             controlnet_negative_prompt_embeds)
         images = _control_tensor(_need(control_images, "control_images", "condition"), self.helper, 2 * batch, 512, 512,
                                  device)
         # 5. latents (:1170-1181): unit noise, scaled by init_noise_sigma inside the loop's prepare()
@@ -391,23 +419,15 @@ class SDXLControlNetAdapterPipeline(DiffusionPipeline):
         else:
             nids = ids
         add_time_ids = torch.cat([nids.repeat(batch, 1), ids.repeat(batch, 1)]).to(device)
-        cscale = controlnet_conditioning_scale
         loop = SDXLControlNetAdapterLoop(
             self.controlnet, self.adapter, self.unet, num_inference_steps=num_inference_steps,
-            guidance_scale=guidance_scale, controlnet_conditioning_scale=cscale[0] if isinstance(cscale, list) else cscale,
-            use_size_512=use_size_512,
-            control_guidance_start=control_guidance_start[0] if isinstance(control_guidance_start, list) else control_guidance_start,
-            control_guidance_end=control_guidance_end[0] if isinstance(control_guidance_end, list) else control_guidance_end)
+            guidance_scale=guidance_scale, controlnet_conditioning_scale=_first(controlnet_conditioning_scale),
+            use_size_512=use_size_512, control_guidance_start=_first(control_guidance_start),
+            control_guidance_end=_first(control_guidance_end))
         loop.prepare(latents=lat, prompt_embeds=torch.cat([negative_prompt_embeds, prompt_embeds]).to(device),
                      add_text_embeds=torch.cat([negative_pooled_prompt_embeds, pooled_prompt_embeds]).to(device),
-                     add_time_ids=add_time_ids,
-                     controlnet_prompt_embeds=torch.cat([controlnet_negative_prompt_embeds,
-                                                         controlnet_prompt_embeds]).to(device),
-                     control_images=images)
-        with self.progress_bar(total=num_inference_steps) as bar:
-            for i in range(num_inference_steps):
-                (loop.step_graph if use_cuda_graph else loop.step)(i)
-                bar.update()
+                     add_time_ids=add_time_ids, controlnet_prompt_embeds=cpe, control_images=images)
+        self._denoise(loop, num_inference_steps, use_cuda_graph)
         latents = loop.latents.to(prompt_embeds.dtype)
         if output_type == "latent":
             image = latents
@@ -488,22 +508,14 @@ class I2VGenXLControlNetAdapterPipeline(DiffusionPipeline):
         # image_embeddings (2B,1,1024) negative first (:808-815); image_latents (2B,4,F,h,w) (:818-833); built from
         # `image` when not passed
         if image is not None and (image_embeddings is None or image_latents is None):
-            emb, lat_img = self.encode_image(image, height, width, f, num_videos_per_prompt, device,
-                                             embeddings=image_embeddings is None, latents=image_latents is None)
-            image_embeddings = emb if image_embeddings is None else image_embeddings
-            image_latents = lat_img if image_latents is None else image_latents
+            image_embeddings, image_latents = _given_or_encoded((image_embeddings, image_latents), self.encode_image(
+                image, height, width, f, num_videos_per_prompt, device, embeddings=image_embeddings is None,
+                latents=image_latents is None))
         image_embeddings = _need(image_embeddings, "image_embeddings (or `image`)", "CLIP vision encoder").to(device)
         image_latents = _need(image_latents, "image_latents (or `image`)", "VAE encoder").to(device)
-        if controlnet_prompt_embeds is None:
-            helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")
-            controlnet_prompt_embeds, controlnet_negative_prompt_embeds, _, _ = helper.encode_controlnet_prompt(
-                prompt, device, 1, True, negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None,
-                lora_scale=None, clip_skip=None)
-        _need(controlnet_negative_prompt_embeds, "controlnet_negative_prompt_embeds", "SD1.5 prompt helper")
         n = 2 * b * f
-        cpe = torch.cat([controlnet_negative_prompt_embeds, controlnet_prompt_embeds]).to(device)
-        if cpe.shape[0] == 2 * b:  # one row per clip -> one per frame-sample (:871-874)
-            cpe = cpe.repeat_interleave(f, dim=0)
+        cpe = _per_frame(self._controlnet_prompt_embeds(prompt, device, controlnet_prompt_embeds,
+                                                        controlnet_negative_prompt_embeds), 2 * b, f)
         multi = isinstance(self.controlnet, MultiControlNetModel)
         _need(control_images, "control_images", "condition")
         if multi:
@@ -522,10 +534,7 @@ class I2VGenXLControlNetAdapterPipeline(DiffusionPipeline):
         loop.prepare(latents=lat, prompt_embeds=torch.cat([negative_prompt_embeds, prompt_embeds]).to(device),
                      image_latents=image_latents, image_embeddings=image_embeddings, fps=fps,
                      controlnet_prompt_embeds=cpe, control_images=images)
-        with self.progress_bar(total=num_inference_steps) as bar:
-            for i in range(num_inference_steps):
-                (loop.step_graph if use_cuda_graph else loop.step)(i)
-                bar.update()
+        self._denoise(loop, num_inference_steps, use_cuda_graph)
         latents = loop.latents_bcfhw().to(prompt_embeds.dtype)
         weights = (None, None)
         if self.router is not None and loop._router_w is not None:  # the reference logs them per step (:990-995)
@@ -611,26 +620,17 @@ class SVDControlNetAdapterPipeline(DiffusionPipeline):
         # image_embeddings (2B,1,1024): zeros for the unconditional half (:497-503); image_latents (2B,F,4,h,w) (:566-583);
         # built from `image` when not passed.  The noise augmentation draws from `generator` before the latents do.
         if image is not None and (image_embeddings is None or image_latents is None):
-            emb, lat_img = self.encode_image(image, height, width, f, num_videos_per_prompt, noise_aug_strength,
-                                             generator, device, embeddings=image_embeddings is None,
-                                             latents=image_latents is None)
-            image_embeddings = emb if image_embeddings is None else image_embeddings
-            image_latents = lat_img if image_latents is None else image_latents
+            image_embeddings, image_latents = _given_or_encoded((image_embeddings, image_latents), self.encode_image(
+                image, height, width, f, num_videos_per_prompt, noise_aug_strength, generator, device,
+                embeddings=image_embeddings is None, latents=image_latents is None))
             # B below is image_embeddings.shape[0] // 2, which now counts every video of every image
             num_videos_per_prompt = 1
         image_embeddings = _need(image_embeddings, "image_embeddings (or `image`)", "CLIP vision encoder").to(device)
         image_latents = _need(image_latents, "image_latents (or `image`)", "VAE encoder").to(device)
         b = image_embeddings.shape[0] // 2
-        if controlnet_prompt_embeds is None:
-            helper = _need(self.helper, "controlnet_prompt_embeds", "SD1.5 prompt helper")
-            controlnet_prompt_embeds, controlnet_negative_prompt_embeds, _, _ = helper.encode_controlnet_prompt(
-                prompt, device, 1, True, negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None,
-                lora_scale=None, clip_skip=None)
-        _need(controlnet_negative_prompt_embeds, "controlnet_negative_prompt_embeds", "SD1.5 prompt helper")
         n = 2 * b * f
-        cpe = torch.cat([controlnet_negative_prompt_embeds, controlnet_prompt_embeds]).to(device)
-        if cpe.shape[0] == 2 * b:
-            cpe = cpe.repeat_interleave(f, dim=0)
+        cpe = _per_frame(self._controlnet_prompt_embeds(prompt, device, controlnet_prompt_embeds,
+                                                        controlnet_negative_prompt_embeds), 2 * b, f)
         images = _control_tensor(_need(control_images, "control_images", "condition"), self.helper, n,
                                  512 if use_size_512 else width, 512 if use_size_512 else height, device)
         # added time ids (:586-596): fps - 1 is what the model was conditioned on during training
@@ -638,20 +638,15 @@ class SVDControlNetAdapterPipeline(DiffusionPipeline):
         added_time_ids = ids.repeat(2 * b * num_videos_per_prompt, 1)
         shape = (b * num_videos_per_prompt, f, 4, height // self.vae_scale_factor, width // self.vae_scale_factor)
         lat = latents.to(device).float() if latents is not None else _randn(shape, generator, device)
-        cs = controlnet_conditioning_scale
         loop = SVDControlNetAdapterLoop(
             self.controlnet, self.adapter, self.unet, num_inference_steps=num_inference_steps,
             min_guidance_scale=min_guidance_scale, max_guidance_scale=max_guidance_scale,
-            controlnet_conditioning_scale=cs[0] if isinstance(cs, list) else cs, use_size_512=use_size_512,
+            controlnet_conditioning_scale=_first(controlnet_conditioning_scale), use_size_512=use_size_512,
             skip_conv_in=skip_conv_in, skip_time_emb=skip_time_emb, sparse_frames=sparse_frames,
-            control_guidance_start=control_guidance_start[0] if isinstance(control_guidance_start, list) else control_guidance_start,
-            control_guidance_end=control_guidance_end[0] if isinstance(control_guidance_end, list) else control_guidance_end)
+            control_guidance_start=_first(control_guidance_start), control_guidance_end=_first(control_guidance_end))
         loop.prepare(latents=lat, image_latents=image_latents, image_embeddings=image_embeddings,
                      added_time_ids=added_time_ids, controlnet_prompt_embeds=cpe, control_images=images)
-        with self.progress_bar(total=num_inference_steps) as bar:
-            for i in range(num_inference_steps):
-                (loop.step_graph if use_cuda_graph else loop.step)(i)
-                bar.update()
+        self._denoise(loop, num_inference_steps, use_cuda_graph)
         latents = loop.latents.to(image_embeddings.dtype)
         if output_type == "latent":
             frames = latents

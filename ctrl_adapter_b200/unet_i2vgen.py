@@ -18,9 +18,9 @@ from torch import nn
 
 from . import ops
 from .persistence import PretrainedMixin
-from .adapter import _ConfigDict, shared_timestep, to_channels_last_bf16
-from .layers import (cache_static_context, BF16, Attention, BasicTransformerBlock, Conv2d, FeedForward, Linear, Norm, Packable, ResnetBlock2D,
-                     TemporalConv, TimestepEmbedding, Transformer2DModel)
+from .layers import (cache_static_context, BF16, Attention, Conv2d, FeedForward, Linear, Norm, Packable, ResnetBlock2D,
+                     TemporalConv, TimestepEmbedding, Transformer2DModel, _ConfigDict, add_residual, add_skip_residuals,
+                     shared_timestep, to_channels_last_bf16)
 from .ops import ACT_SILU
 
 
@@ -185,19 +185,6 @@ class _LatentTemporalEncoder(Packable):
         return ops.i2vgen_latent_encoder(x, clips, frames, self.packed())
 
 
-class _ConvPad8(Conv2d):
-    """Conv whose output channel count (4) is zero padded to 8 for the 16-byte vector stores."""
-
-    def pack(self):
-        w, b = super().pack()
-        co = w.shape[0]
-        cp = (co + 7) // 8 * 8
-        if cp != co:
-            w = torch.cat([w, torch.zeros(cp - co, w.shape[1], device=w.device, dtype=w.dtype)], 0).contiguous()
-            b = torch.cat([b, torch.zeros(cp - co, device=b.device, dtype=b.dtype)]).contiguous()
-        return w, b
-
-
 class I2VGenXLUNet(PretrainedMixin, nn.Module):
     def __init__(self, sample_size=None, in_channels: int = 4, out_channels: int = 4,
                  down_block_types=("CrossAttnDownBlock3D", "CrossAttnDownBlock3D", "CrossAttnDownBlock3D", "DownBlock3D"),
@@ -215,7 +202,7 @@ class I2VGenXLUNet(PretrainedMixin, nn.Module):
         temb = c[0] * 4
         self.conv_in = Conv2d(2 * in_channels, c[0], 3)
         self.transformer_in = TransformerTemporalModel(8, 64, c[0])
-        self.image_latents_proj_in = _Seq(_0=Conv2d(4, 16, 3), _2=Conv2d(16, 16, 3), _4=_ConvPad8(16, 4, 3))
+        self.image_latents_proj_in = _Seq(_0=Conv2d(4, 16, 3), _2=Conv2d(16, 16, 3), _4=Conv2d(16, 4, 3))
         self.image_latents_temporal_encoder = _LatentTemporalEncoder(4)
         self.image_latents_context_embedding = _Seq(_0=Conv2d(4, 32, 3), _3=Conv2d(32, 64, 3, stride=2),
                                                     _5=Conv2d(64, cross_attention_dim, 3, stride=2))
@@ -234,16 +221,8 @@ class I2VGenXLUNet(PretrainedMixin, nn.Module):
             _Block3D("up", c[0], c[1], c[2], temb, cross_attention_dim, True, 3, "up"),
             _Block3D("up", c[0], c[0], c[1], temb, cross_attention_dim, True, 3, None)])
         self.conv_norm_out = Norm(c[0], 1e-5)
-        self.conv_out = _ConvPad8(c[0], out_channels, 3)
+        self.conv_out = Conv2d(c[0], out_channels, 3)
         self._cond_cache = None
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
 
     # ------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -304,22 +283,14 @@ class I2VGenXLUNet(PretrainedMixin, nn.Module):
         for blk in self.down_blocks:
             x, outs = blk(x, temb_act, ctx, f, kv_div=f)
             skips += outs
-        if down_block_additional_residuals is not None:
-            for i, (s_, r) in enumerate(zip(skips, down_block_additional_residuals)):
-                skips[i] = ops.add(s_, _residual_nhwc(r))
+        if down_block_additional_residuals is not None:  # 4-D or 5-D residuals (reference :681-695, :709-714)
+            add_skip_residuals(skips, down_block_additional_residuals)
         x = self.mid_block(x, temb_act, ctx, f, kv_div=f)
         if mid_block_additional_residual is not None:
-            x = ops.add(x, _residual_nhwc(mid_block_additional_residual))
+            x = add_residual(x, mid_block_additional_residual)
         for blk in self.up_blocks:
             x = blk(x, temb_act, ctx, f, skips=skips, kv_div=f)
         y = self.conv_out(self.conv_norm_out.group_norm(x, silu=True))         # [n, h, w, 8]
         out = ops.nhwc_to_nchw(y, ch)                                          # (b f) c h w
         return (out.reshape(b, f, ch, h, w).permute(0, 2, 1, 3, 4),)
 
-
-def _residual_nhwc(r: torch.Tensor) -> torch.Tensor:
-    """adapter residual, 4-D (b f) c h w or 5-D b c f h w (reference :682-683) -> [b*f, h, w, c] bf16."""
-    if r.dim() == 5:
-        b, c, f, h, w = r.shape
-        r = r.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
-    return to_channels_last_bf16(r)

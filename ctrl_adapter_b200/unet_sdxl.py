@@ -7,83 +7,33 @@ consumed as a second TMA source of the up-block convolutions / GroupNorms, so ``
 """
 from __future__ import annotations
 
-from typing import Optional
-
 import torch
 from torch import nn
 
 from . import ops
 from .persistence import PretrainedMixin
-from .adapter import _ConfigDict, as_nchw, shared_timestep, to_channels_last_bf16
-from .layers import BF16, Conv2d, Norm, ResnetBlock2D, TimestepEmbedding, Transformer2DModel
+from .layers import (BF16, Conv2d, DownBlock2D, MidBlock2D, Norm, ResnetBlock2D, TimestepEmbedding, Transformer2DModel,
+                     UpBlock2D, _ConfigDict, add_residual, add_skip_residuals, shared_timestep, to_channels_last_bf16)
 
 
-class _Down(nn.Module):
-    def __init__(self, cin, cout, temb, eps, heads, depth, cross_dim, add_downsample):
-        super().__init__()
-        self.has_cross_attention = depth > 0
-        self.resnets = nn.ModuleList([ResnetBlock2D(cin if i == 0 else cout, cout, temb, eps) for i in range(2)])
-        if depth > 0:
-            self.attentions = nn.ModuleList([Transformer2DModel(heads, cout // heads, cout, depth, cross_dim, True)
-                                             for _ in range(2)])
-        self.downsamplers = None
-        if add_downsample:
-            ds = nn.Module()
-            ds.conv = Conv2d(cout, cout, 3, stride=2)
-            self.downsamplers = nn.ModuleList([ds])
-
-    def forward(self, x, temb_act, ctx):
-        outs = []
-        for i, r in enumerate(self.resnets):
-            x = r(x, temb_act)
-            if self.has_cross_attention:
-                x = self.attentions[i](x, ctx)
-            outs.append(x)
-        if self.downsamplers is not None:
-            x = self.downsamplers[0].conv(x)
-            outs.append(x)
-        return x, outs
+def _attentions(n, heads, c, depth, cross_dim):
+    if depth == 0:
+        return None
+    return [Transformer2DModel(heads, c // heads, c, depth, cross_dim, True) for _ in range(n)]
 
 
-class _Mid(nn.Module):
-    def __init__(self, c, temb, eps, heads, depth, cross_dim):
-        super().__init__()
-        self.resnets = nn.ModuleList([ResnetBlock2D(c, c, temb, eps), ResnetBlock2D(c, c, temb, eps)])
-        self.attentions = nn.ModuleList([Transformer2DModel(heads, c // heads, c, depth, cross_dim, True)])
-
-    def forward(self, x, temb_act, ctx):
-        x = self.resnets[0](x, temb_act)
-        x = self.attentions[0](x, ctx)
-        return self.resnets[1](x, temb_act)
+def _down(cin, cout, temb, eps, heads, depth, cross_dim, add_downsample):
+    return DownBlock2D([ResnetBlock2D(cin if i == 0 else cout, cout, temb, eps) for i in range(2)],
+                       _attentions(2, heads, cout, depth, cross_dim),
+                       Conv2d(cout, cout, 3, stride=2) if add_downsample else None)
 
 
-class _Up(nn.Module):
-    def __init__(self, cin, cout, prev, temb, eps, heads, depth, cross_dim, add_upsample):
-        super().__init__()
-        self.has_cross_attention = depth > 0
-        rs = []
-        for i in range(3):
-            skip_c = cin if i == 2 else cout
-            in_c = prev if i == 0 else cout
-            rs.append(ResnetBlock2D(in_c + skip_c, cout, temb, eps))
-        self.resnets = nn.ModuleList(rs)
-        if depth > 0:
-            self.attentions = nn.ModuleList([Transformer2DModel(heads, cout // heads, cout, depth, cross_dim, True)
-                                             for _ in range(3)])
-        self.upsamplers = None
-        if add_upsample:
-            us = nn.Module()
-            us.conv = Conv2d(cout, cout, 3)
-            self.upsamplers = nn.ModuleList([us])
-
-    def forward(self, x, skips, temb_act, ctx):
-        for i, r in enumerate(self.resnets):
-            x = r(x, temb_act, x2=skips.pop())
-            if self.has_cross_attention:
-                x = self.attentions[i](x, ctx)
-        if self.upsamplers is not None:
-            x = self.upsamplers[0].conv(ops.upsample2x(x))
-        return x
+def _up(cin, cout, prev, temb, eps, heads, depth, cross_dim, add_upsample):
+    # resnet i: the previous output (prev, then cout channels) + the skip it pops (cout, cout, then cin channels)
+    return UpBlock2D([ResnetBlock2D((prev if i == 0 else cout) + (cin if i == 2 else cout), cout, temb, eps)
+                      for i in range(3)],
+                     _attentions(3, heads, cout, depth, cross_dim),
+                     Conv2d(cout, cout, 3) if add_upsample else None)
 
 
 class UNet2DConditionModel(PretrainedMixin, nn.Module):
@@ -101,45 +51,25 @@ class UNet2DConditionModel(PretrainedMixin, nn.Module):
         c0, c1, c2 = block_out_channels
         temb = c0 * 4
         heads = tuple(attention_head_dim)
+        depth = transformer_layers_per_block
+        xd = cross_attention_dim
         self.flip_sin_to_cos, self.freq_shift = flip_sin_to_cos, freq_shift
         self.conv_in = Conv2d(in_channels, c0, 3)
         self.time_embedding = TimestepEmbedding(c0, temb)
         self.add_embedding = TimestepEmbedding(projection_class_embeddings_input_dim, temb)
         # down: DownBlock2D, CrossAttnDownBlock2D(depth 2), CrossAttnDownBlock2D(depth 10)
         self.down_blocks = nn.ModuleList([
-            _Down(c0, c0, temb, norm_eps, heads[0], 0, cross_attention_dim, True),
-            _Down(c0, c1, temb, norm_eps, heads[1], transformer_layers_per_block[1], cross_attention_dim, True),
-            _Down(c1, c2, temb, norm_eps, heads[2], transformer_layers_per_block[2], cross_attention_dim, False)])
-        self.mid_block = _Mid(c2, temb, norm_eps, heads[2], transformer_layers_per_block[2], cross_attention_dim)
+            _down(c0, c0, temb, norm_eps, heads[0], 0, xd, True),
+            _down(c0, c1, temb, norm_eps, heads[1], depth[1], xd, True),
+            _down(c1, c2, temb, norm_eps, heads[2], depth[2], xd, False)])
+        self.mid_block = MidBlock2D([ResnetBlock2D(c2, c2, temb, norm_eps), ResnetBlock2D(c2, c2, temb, norm_eps)],
+                                    [Transformer2DModel(heads[2], c2 // heads[2], c2, depth[2], xd, True)])
         self.up_blocks = nn.ModuleList([
-            _Up(c1, c2, c2, temb, norm_eps, heads[2], transformer_layers_per_block[2], cross_attention_dim, True),
-            _Up(c0, c1, c2, temb, norm_eps, heads[1], transformer_layers_per_block[1], cross_attention_dim, True),
-            _Up(c0, c0, c1, temb, norm_eps, heads[0], 0, cross_attention_dim, False)])
+            _up(c1, c2, c2, temb, norm_eps, heads[2], depth[2], xd, True),
+            _up(c0, c1, c2, temb, norm_eps, heads[1], depth[1], xd, True),
+            _up(c0, c0, c1, temb, norm_eps, heads[0], 0, xd, False)])
         self.conv_norm_out = Norm(c0, norm_eps)
         self.conv_out = Conv2d(c0, out_channels, 3)
-        self._conv_out_pad = None
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
-    def _conv_out_packed(self):
-        """conv_out has 4 output channels; the kernel stores 16-byte vectors, so its weight rows are zero padded to 8."""
-        key = self.conv_out._key()
-        if self._conv_out_pad is None or self._conv_out_pad[0] != key:
-            w, b = self.conv_out.packed()
-            co = w.shape[0]
-            cp = (co + 7) // 8 * 8
-            wp = torch.zeros((cp, w.shape[1]), device=w.device, dtype=w.dtype)
-            wp[:co] = w
-            bp = torch.zeros(cp, device=w.device, dtype=torch.float32)
-            bp[:co] = b
-            self._conv_out_pad = (key, wp, bp)
-        return self._conv_out_pad[1], self._conv_out_pad[2]
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, timestep_cond=None, cross_attention_kwargs=None,
@@ -169,16 +99,12 @@ class UNet2DConditionModel(PretrainedMixin, nn.Module):
             x, outs = blk(x, temb_act, ctx)
             skips += outs
         is_controlnet = mid_block_additional_residual is not None and down_block_additional_residuals is not None
-        if is_controlnet:  # zip() truncation: only the first 9 of the adapter's 12 tensors are consumed
-            for i, (s, r) in enumerate(zip(skips, down_block_additional_residuals)):
-                skips[i] = ops.add(s, to_channels_last_bf16(r))
+        if is_controlnet:  # only the first 9 of the adapter's 12 tensors are consumed
+            add_skip_residuals(skips, down_block_additional_residuals)
         x = self.mid_block(x, temb_act, ctx)
         if is_controlnet and isinstance(mid_block_additional_residual, torch.Tensor):
-            x = ops.add(x, to_channels_last_bf16(mid_block_additional_residual))
+            x = add_residual(x, mid_block_additional_residual)
         for blk in self.up_blocks:
-            x = blk(x, skips, temb_act, ctx)
-        h = self.conv_norm_out.group_norm(x, silu=True)
-        w, b = self._conv_out_packed()
-        y = ops.conv2d(h, w, b, ksize=3)
-        out = ops.nhwc_to_nchw(y, self.config.out_channels)
-        return (out,)
+            x = blk(x, temb_act, ctx, skips=skips)
+        y = self.conv_out(self.conv_norm_out.group_norm(x, silu=True))          # [n, h, w, 8]
+        return (ops.nhwc_to_nchw(y, self.config.out_channels),)

@@ -20,9 +20,10 @@ from torch import nn
 
 from . import ops
 from .persistence import PretrainedMixin
-from .adapter import (AlphaBlender, TemporalBasicTransformerBlock, TemporalResnetBlock, _ConfigDict, shared_timestep,
-                      to_channels_last_bf16)
-from .layers import BF16, BasicTransformerBlock, Conv2d, Linear, Norm, ResnetBlock2D, TimestepEmbedding
+from .adapter import AlphaBlender, TemporalBasicTransformerBlock, TemporalResnetBlock
+from .layers import (BF16, BasicTransformerBlock, Conv2d, DownBlock2D, Linear, MidBlock2D, Norm, ResnetBlock2D,
+                     TimestepEmbedding, UpBlock2D, _ConfigDict, add_residual, add_skip_residuals, shared_timestep,
+                     to_channels_last_bf16)
 
 
 class SpatioTemporalResBlock(nn.Module):
@@ -81,73 +82,21 @@ class TransformerSpatioTemporalModel(nn.Module):
 
 
 def _transformers(n, heads, c, depth, cross_dim):
-    return nn.ModuleList([TransformerSpatioTemporalModel(heads, c // heads, c, depth, cross_dim) for _ in range(n)])
+    return [TransformerSpatioTemporalModel(heads, c // heads, c, depth, cross_dim) for _ in range(n)]
 
 
-class _Down(nn.Module):
-    def __init__(self, cin, cout, temb, eps, heads, depth, cross_dim, add_downsample, cross_attn):
-        super().__init__()
-        self.has_cross_attention = cross_attn
-        self.resnets = nn.ModuleList([SpatioTemporalResBlock(cin if i == 0 else cout, cout, temb, eps) for i in range(2)])
-        if cross_attn:
-            self.attentions = _transformers(2, heads, cout, depth, cross_dim)
-        self.downsamplers = None
-        if add_downsample:
-            ds = nn.Module()
-            ds.conv = Conv2d(cout, cout, 3, stride=2)
-            self.downsamplers = nn.ModuleList([ds])
-
-    def forward(self, x, temb_act, ctx_vecs, frames):
-        outs = []
-        for i, r in enumerate(self.resnets):
-            x = r(x, temb_act, frames)
-            if self.has_cross_attention:
-                x = self.attentions[i](x, ctx_vecs, frames)
-            outs.append(x)
-        if self.downsamplers is not None:
-            x = self.downsamplers[0].conv(x)
-            outs.append(x)
-        return x, outs
+def _down(cin, cout, temb, eps, heads, depth, cross_dim, add_downsample, cross_attn):
+    return DownBlock2D([SpatioTemporalResBlock(cin if i == 0 else cout, cout, temb, eps) for i in range(2)],
+                       _transformers(2, heads, cout, depth, cross_dim) if cross_attn else None,
+                       Conv2d(cout, cout, 3, stride=2) if add_downsample else None)
 
 
-class _Mid(nn.Module):
-    def __init__(self, c, temb, heads, depth, cross_dim):
-        super().__init__()
-        self.resnets = nn.ModuleList([SpatioTemporalResBlock(c, c, temb, 1e-5), SpatioTemporalResBlock(c, c, temb, 1e-5)])
-        self.attentions = _transformers(1, heads, c, depth, cross_dim)
-
-    def forward(self, x, temb_act, ctx_vecs, frames):
-        x = self.resnets[0](x, temb_act, frames)
-        x = self.attentions[0](x, ctx_vecs, frames)
-        return self.resnets[1](x, temb_act, frames)
-
-
-class _Up(nn.Module):
-    def __init__(self, cin, cout, prev, temb, eps, heads, depth, cross_dim, add_upsample, cross_attn):
-        super().__init__()
-        self.has_cross_attention = cross_attn
-        rs = []
-        for i in range(3):
-            skip_c = cin if i == 2 else cout
-            in_c = prev if i == 0 else cout
-            rs.append(SpatioTemporalResBlock(in_c + skip_c, cout, temb, eps))
-        self.resnets = nn.ModuleList(rs)
-        if cross_attn:
-            self.attentions = _transformers(3, heads, cout, depth, cross_dim)
-        self.upsamplers = None
-        if add_upsample:
-            us = nn.Module()
-            us.conv = Conv2d(cout, cout, 3)
-            self.upsamplers = nn.ModuleList([us])
-
-    def forward(self, x, skips, temb_act, ctx_vecs, frames):
-        for i, r in enumerate(self.resnets):
-            x = r(x, temb_act, frames, x2=skips.pop())
-            if self.has_cross_attention:
-                x = self.attentions[i](x, ctx_vecs, frames)
-        if self.upsamplers is not None:
-            x = self.upsamplers[0].conv(ops.upsample2x(x))
-        return x
+def _up(cin, cout, prev, temb, eps, heads, depth, cross_dim, add_upsample, cross_attn):
+    # resnet i: the previous output (prev, then cout channels) + the skip it pops (cout, cout, then cin channels)
+    return UpBlock2D([SpatioTemporalResBlock((prev if i == 0 else cout) + (cin if i == 2 else cout), cout, temb, eps)
+                      for i in range(3)],
+                     _transformers(3, heads, cout, depth, cross_dim) if cross_attn else None,
+                     Conv2d(cout, cout, 3) if add_upsample else None)
 
 
 class UNetSpatioTemporalConditionModel(PretrainedMixin, nn.Module):
@@ -190,46 +139,19 @@ class UNetSpatioTemporalConditionModel(PretrainedMixin, nn.Module):
         # class-default eps of diffusers v0.27.2 (get_down_block / get_up_block do not forward resnet_eps to these types)
         h0, h1, h2, h3 = heads
         self.down_blocks = nn.ModuleList([
-            _Down(c0, c0, temb, 1e-6, h0, 1, xd, True, True),
-            _Down(c0, c1, temb, 1e-6, h1, 1, xd, True, True),
-            _Down(c1, c2, temb, 1e-6, h2, 1, xd, True, True),
-            _Down(c2, c3, temb, 1e-5, h3, 1, xd, False, False)])
-        self.mid_block = _Mid(c3, temb, h3, 1, xd)
+            _down(c0, c0, temb, 1e-6, h0, 1, xd, True, True),
+            _down(c0, c1, temb, 1e-6, h1, 1, xd, True, True),
+            _down(c1, c2, temb, 1e-6, h2, 1, xd, True, True),
+            _down(c2, c3, temb, 1e-5, h3, 1, xd, False, False)])
+        self.mid_block = MidBlock2D([SpatioTemporalResBlock(c3, c3, temb, 1e-5) for _ in range(2)],
+                                    _transformers(1, h3, c3, 1, xd))
         self.up_blocks = nn.ModuleList([
-            _Up(c2, c3, c3, temb, 1e-6, h3, 1, xd, True, False),
-            _Up(c1, c2, c3, temb, 1e-6, h2, 1, xd, True, True),
-            _Up(c0, c1, c2, temb, 1e-6, h1, 1, xd, True, True),
-            _Up(c0, c0, c1, temb, 1e-6, h0, 1, xd, False, True)])
+            _up(c2, c3, c3, temb, 1e-6, h3, 1, xd, True, False),
+            _up(c1, c2, c3, temb, 1e-6, h2, 1, xd, True, True),
+            _up(c0, c1, c2, temb, 1e-6, h1, 1, xd, True, True),
+            _up(c0, c0, c1, temb, 1e-6, h0, 1, xd, False, True)])
         self.conv_norm_out = Norm(c0, 1e-5)
         self.conv_out = Conv2d(c0, out_channels, 3)
-        self._conv_out_pad = None
-
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
-    def _conv_out_packed(self):
-        """conv_out has 4 output channels; the kernel stores 16-byte vectors, so its weight rows are zero padded to 8."""
-        key = self.conv_out._key()
-        if self._conv_out_pad is None or self._conv_out_pad[0] != key:
-            w, b = self.conv_out.packed()
-            co = w.shape[0]
-            cp = (co + 7) // 8 * 8
-            wp = torch.zeros((cp, w.shape[1]), device=w.device, dtype=w.dtype)
-            wp[:co] = w
-            bp = torch.zeros(cp, device=w.device, dtype=torch.float32)
-            bp[:co] = b
-            self._conv_out_pad = (key, wp, bp)
-        return self._conv_out_pad[1], self._conv_out_pad[2]
-
-    @staticmethod
-    def _flatten_frames(r: torch.Tensor) -> torch.Tensor:
-        """5-D "b c f h w" residual -> (b f) c h w (unet_spatio_temporal_condition.py:459, 487)."""
-        return r.permute(0, 2, 1, 3, 4).flatten(0, 1) if r.dim() == 5 else r
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, added_time_ids, down_block_additional_residuals=None,
@@ -258,17 +180,14 @@ class UNetSpatioTemporalConditionModel(PretrainedMixin, nn.Module):
         for blk in self.down_blocks:
             x, outs = blk(x, temb_act, ctx_vecs, f)
             skips += outs
-        if down_block_additional_residuals is not None:  # zip() truncation to the shorter list (:463-468)
-            for i, (s, r) in enumerate(zip(skips, down_block_additional_residuals)):
-                skips[i] = ops.add(s, to_channels_last_bf16(self._flatten_frames(r)))
+        if down_block_additional_residuals is not None:  # 4-D or 5-D residuals (:457-471, :485-490)
+            add_skip_residuals(skips, down_block_additional_residuals)
         x = self.mid_block(x, temb_act, ctx_vecs, f)
         if isinstance(mid_block_additional_residual, torch.Tensor):
-            x = ops.add(x, to_channels_last_bf16(self._flatten_frames(mid_block_additional_residual)))
+            x = add_residual(x, mid_block_additional_residual)
         for blk in self.up_blocks:
-            x = blk(x, skips, temb_act, ctx_vecs, f)
-        h = self.conv_norm_out.group_norm(x, silu=True)
-        w, bias = self._conv_out_packed()
-        y = ops.conv2d(h, w, bias, ksize=3)
+            x = blk(x, temb_act, ctx_vecs, f, skips=skips)
+        y = self.conv_out(self.conv_norm_out.group_norm(x, silu=True))         # [B*F, H, W, 8]
         out = ops.nhwc_to_nchw(y, self.config.out_channels)  # [B*F, 4, H, W]
         out = out.reshape(b, f, *out.shape[1:])
         return (out,)

@@ -27,8 +27,8 @@ import torch
 from torch import nn
 
 from . import ops
-from .adapter import AlphaBlender, TemporalResnetBlock, _ConfigDict, as_nchw, to_channels_last_bf16
-from .layers import BF16, Conv2d, Linear, Norm, Packable, ResnetBlock2D
+from .adapter import AlphaBlender, TemporalResnetBlock
+from .layers import BF16, Conv2d, Linear, Norm, Packable, ResnetBlock2D, _ConfigDict, to_channels_last_bf16
 from .persistence import PretrainedMixin
 
 
@@ -103,28 +103,13 @@ class Decoder(nn.Module):
         self.conv_norm_out = Norm(rev[-1], eps)
         self.conv_out = Conv2d(rev[-1], out_channels, 3)
         self.out_channels = out_channels
-        self._conv_out_pad = None
-
-    def _conv_out_packed(self):
-        """conv_out has 3 output channels; the kernel stores 16-byte vectors, so its weight rows are zero padded to 8."""
-        key = self.conv_out._key()
-        if self._conv_out_pad is None or self._conv_out_pad[0] != key:
-            w, b = self.conv_out.packed()
-            wp = torch.zeros((8, w.shape[1]), device=w.device, dtype=w.dtype)
-            wp[: w.shape[0]] = w
-            bp = torch.zeros(8, device=w.device, dtype=torch.float32)
-            bp[: b.shape[0]] = b
-            self._conv_out_pad = (key, wp, bp)
-        return self._conv_out_pad[1], self._conv_out_pad[2]
 
     def forward(self, z_nhwc8):
         x = self.conv_in(z_nhwc8)
         x = self.mid_block(x)
         for blk in self.up_blocks:
             x = blk(x)
-        x = self.conv_norm_out.group_norm(x, silu=True)
-        w, b = self._conv_out_packed()
-        return ops.conv2d(x, w, b, ksize=3)  # [n, H, W, 8], the first out_channels are real
+        return self.conv_out(self.conv_norm_out.group_norm(x, silu=True))  # [n, H, W, 8], the first out_channels are real
 
 
 class DecoderOutput:
@@ -241,14 +226,6 @@ class _KLVae(PretrainedMixin, nn.Module):
         self.quant_conv = Conv2d(2 * latent_channels, 2 * latent_channels, 1)
         self.encoder_loaded = True
 
-    @property
-    def dtype(self):
-        return next(self.parameters()).dtype
-
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         own = {k: tuple(v.shape) for k, v in self.state_dict().items() if k.startswith(self.encoder_prefixes)}
         complete = all(k in state_dict and tuple(state_dict[k].shape) == s for k, s in own.items())
@@ -307,17 +284,7 @@ class AutoencoderKL(_KLVae):
         """z [N, 4, h, w] (already divided by scaling_factor by the caller, as the pipelines do) -> images [N, 3, 8h, 8w]
         in [-1, 1] (logical NCHW, bf16)."""
         x = to_channels_last_bf16(z.to(BF16) if z.dtype not in (BF16, torch.float32) else z, 8)  # 4 -> 8 zero-padded channels
-        w, b = self.post_quant_conv.packed()
-        # 1x1 conv 4 -> 4 on the padded layout: output rows padded to 8 as well
-        key = self.post_quant_conv._key()
-        if getattr(self, "_pq_pad", None) is None or self._pq_pad[0] != key:
-            wp = torch.zeros((8, w.shape[1]), device=w.device, dtype=w.dtype)
-            wp[: w.shape[0]] = w
-            bp = torch.zeros(8, device=w.device, dtype=torch.float32)
-            bp[: b.shape[0]] = b
-            self._pq_pad = (key, wp, bp)
-        x = ops.conv2d(x, self._pq_pad[1], self._pq_pad[2], ksize=1)
-        y = self.decoder(x)
+        y = self.decoder(self.post_quant_conv(x))  # 1x1 conv 4 -> 4 on the padded layout: [n, h, w, 8]
         img = ops.nhwc_to_nchw(y, self.config.out_channels)
         return DecoderOutput(img) if return_dict else (img,)
 
@@ -405,9 +372,6 @@ class TemporalDecoder(nn.Module):
         self.conv_norm_out = Norm(rev[-1], 1e-6)
         self.conv_out = Conv2d(rev[-1], out_channels, 3)
         self.time_conv_out = _FrameConvSmall(out_channels)
-        self._conv_out_pad = None
-
-    _conv_out_packed = Decoder._conv_out_packed
 
     def forward(self, z_nhwc8, frames: int):
         """z [B*F, h, w, 8] (frames of a clip contiguous) -> images [B*F, 3, 8h, 8w] bf16 (logical NCHW)."""
@@ -415,9 +379,7 @@ class TemporalDecoder(nn.Module):
         x = self.mid_block(x, frames)
         for blk in self.up_blocks:
             x = blk(x, frames)
-        x = self.conv_norm_out.group_norm(x, silu=True)
-        w, b = self._conv_out_packed()
-        y = ops.conv2d(x, w, b, ksize=3)                       # [n, H, W, 8], the first out_channels are real
+        y = self.conv_out(self.conv_norm_out.group_norm(x, silu=True))  # [n, H, W, 8], the first out_channels are real
         return self.time_conv_out(y, frames)
 
 

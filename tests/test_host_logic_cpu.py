@@ -104,13 +104,14 @@ def test_router_state_dict_and_config():
         A.ControlNetRouter(router_type="sparsemax")
 
 
-def test_timestep_forms():
+def test_timestep_vector_forms():
+    from ctrl_adapter_b200.layers import timestep_vector
     dev = torch.device("cpu")
     for t in (981, 981.0, torch.tensor(981.0), torch.tensor([981.0]), torch.tensor([[981.0], [981.0], [981.0]])):
-        v = A.timestep_vector(t, 3, dev)
+        v = timestep_vector(t, 3, dev)
         assert v.shape == (3,) and v.dtype == torch.float32 and float(v[0]) == 981.0
     with pytest.raises(TypeError):
-        A.timestep_vector("981", 3, dev)
+        timestep_vector("981", 3, dev)
 
 
 def test_adapter_rejects_unsupported_configs():
