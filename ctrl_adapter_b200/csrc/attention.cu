@@ -320,6 +320,14 @@ extern "C" int ca_attention(const ca_attention_desc* d, void* cuda_stream) {
   if (d->batch < 1 || d->heads < 1 || d->lq < 1 || d->lk < 1) return fail(CA_ERR_INVALID, "empty attention problem");
   const int kv_div = d->kv_batch_div > 0 ? d->kv_batch_div : 1;
   if (d->batch % kv_div != 0) return fail(CA_ERR_INVALID, "batch must be a multiple of kv_batch_div");
+  // grid (q tiles, heads * head_dim_pad / 64, batch)
+  if (d->batch > kMaxGridYZ) return fail(CA_ERR_INVALID, "batch (%d) must be <= 65535", d->batch);
+  if (static_cast<long long>(d->heads) * (d->head_dim_pad / 64) > kMaxGridYZ)
+    return fail(CA_ERR_INVALID, "heads * head_dim_pad / 64 (%d * %d) must be <= 65535", d->heads, d->head_dim_pad / 64);
+  // the epilogue stores bf16 pairs as 4-byte words
+  if (!aligned(d->out, 4) || (d->out_row_stride & 1) != 0 || (d->out_batch_stride & 1) != 0)
+    return fail(CA_ERR_INVALID, "out must be 4-byte aligned with even out_row_stride, out_batch_stride (%lld, %lld)",
+                (long long)d->out_row_stride, (long long)d->out_batch_stride);
   const cuuint64_t ctot = static_cast<cuuint64_t>(d->heads) * d->head_dim_pad;
   CUtensorMap tq, tk, tv;
   const cuuint32_t box[3] = {64, 128, 1};

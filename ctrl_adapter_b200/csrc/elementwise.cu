@@ -39,6 +39,9 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, int n, in
 }
 extern "C" int ca_timestep_embedding(const float* t, int32_t n, int32_t dim, int32_t flip_sin_to_cos, float freq_shift,
                                      int32_t round_t_bf16, void* out, void* s) {
+  // dim 1 has no sinusoid pair: the kernel would never write its one (zero) column
+  if (dim < 2) return fail(CA_ERR_INVALID, "timestep_embedding: dim (%d) must be >= 2", dim);
+  if (n < 1) return fail(CA_ERR_INVALID, "timestep_embedding: n (%d) must be positive", n);
   const long long total = static_cast<long long>(n) * (dim / 2);
   return launched(launch_pdl(timestep_embedding_kernel, blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(s), t,
                              n, dim, flip_sin_to_cos, freq_shift, round_t_bf16, static_cast<__nv_bfloat16*>(out)),
@@ -63,6 +66,7 @@ __global__ void silu_kernel(const uint4* __restrict__ x, long long nvec, uint4* 
 }
 extern "C" int ca_silu(const void* x, int64_t n, void* y, void* s) {
   if (n & 7) return fail(CA_ERR_INVALID, "silu: n (%lld) must be a multiple of 8", (long long)n);
+  if (!aligned(x, 16) || !aligned(y, 16)) return fail(CA_ERR_INVALID, "silu: x, y must be 16-byte aligned");
   return launched(launch_pdl(silu_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s),
                              static_cast<const uint4*>(x), n / 8, static_cast<uint4*>(y)),
                   "silu");
@@ -88,6 +92,8 @@ __global__ void add_kernel(const uint4* __restrict__ a, const uint4* __restrict_
 }
 extern "C" int ca_add(const void* a, const void* b, int64_t n, void* y, void* s) {
   if (n & 7) return fail(CA_ERR_INVALID, "add: n (%lld) must be a multiple of 8", (long long)n);
+  if (!aligned(a, 16) || !aligned(b, 16) || !aligned(y, 16))
+    return fail(CA_ERR_INVALID, "add: a, b, y must be 16-byte aligned");
   return launched(launch_pdl(add_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s),
                              static_cast<const uint4*>(a), static_cast<const uint4*>(b), n / 8, static_cast<uint4*>(y)),
                   "add");
@@ -121,6 +127,13 @@ __global__ void nchw_to_nhwc_kernel(const SrcT* __restrict__ x, int c, long long
 }
 extern "C" int ca_nchw_to_nhwc(const void* x, int32_t src_fp32, int32_t n, int32_t c, int64_t hw, int32_t c_pad,
                                void* y_, void* s) {
+  if (n < 1 || c < 1 || hw < 1) return fail(CA_ERR_INVALID, "nchw_to_nhwc: n, c, hw (%d, %d, %lld) must be positive", n, c,
+                                            (long long)hw);
+  // c > c_pad would drop channels without a word
+  if (c_pad < c) return fail(CA_ERR_INVALID, "nchw_to_nhwc: c_pad (%d) must be >= c (%d)", c_pad, c);
+  if (n > kMaxGridYZ || (static_cast<long long>(c_pad) + 31) / 32 > kMaxGridYZ || hw > 0xffffffffLL)
+    return fail(CA_ERR_INVALID, "nchw_to_nhwc: n (%d) must be <= 65535, c_pad (%d) <= 65535 * 32 and hw (%lld) < 2^32",
+                n, c_pad, (long long)hw);
   const dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c_pad + 31) / 32, n), block(32, 8);
   cudaStream_t stream = static_cast<cudaStream_t>(s);
   __nv_bfloat16* y = static_cast<__nv_bfloat16*>(y_);
@@ -155,6 +168,13 @@ __global__ void nhwc_to_nchw_kernel(const __nv_bfloat16* __restrict__ x, int c, 
 }
 extern "C" int ca_nhwc_to_nchw(const void* x_, int32_t n, int32_t c, int32_t c_stride, int64_t hw, void* y,
                                int32_t dst_fp32, void* s) {
+  if (n < 1 || c < 1 || hw < 1) return fail(CA_ERR_INVALID, "nhwc_to_nchw: n, c, hw (%d, %d, %lld) must be positive", n, c,
+                                            (long long)hw);
+  // c > c_stride would read channel c_stride.. from the next pixel
+  if (c_stride < c) return fail(CA_ERR_INVALID, "nhwc_to_nchw: c_stride (%d) must be >= c (%d)", c_stride, c);
+  if (n > kMaxGridYZ || (static_cast<long long>(c) + 31) / 32 > kMaxGridYZ || hw > 0xffffffffLL)
+    return fail(CA_ERR_INVALID, "nhwc_to_nchw: n (%d) must be <= 65535, c (%d) <= 65535 * 32 and hw (%lld) < 2^32", n, c,
+                (long long)hw);
   const dim3 grid(static_cast<unsigned>((hw + 31) / 32), (c + 31) / 32, n), block(32, 8);
   cudaStream_t stream = static_cast<cudaStream_t>(s);
   const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(x_);
@@ -217,6 +237,7 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, int h, int w, int
 }
 extern "C" int ca_upsample2x(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, void* y, void* s) {
   if (c & 7) return fail(CA_ERR_INVALID, "upsample2x: c (%d) must be a multiple of 8", c);
+  if (!aligned(x, 16) || !aligned(y, 16)) return fail(CA_ERR_INVALID, "upsample2x: x, y must be 16-byte aligned");
   const long long total = static_cast<long long>(n) * h * w * (c / 8);
   return launched(launch_pdl(upsample2x_kernel, blocks_for(total, 256), 256, 0, static_cast<cudaStream_t>(s),
                              static_cast<const uint4*>(x), h, w, c / 8, total, static_cast<uint4*>(y)),
@@ -250,6 +271,7 @@ __global__ void router_weights_kernel(const float* __restrict__ logits, const un
 extern "C" int ca_router_weights(const float* logits, const uint8_t* mask, int32_t nrouters, int32_t nexperts,
                                  float* weights, void* s) {
   if (nexperts < 1 || nexperts > 32) return fail(CA_ERR_INVALID, "router_weights: nexperts must be 1..32 (got %d)", nexperts);
+  if (nrouters < 1) return fail(CA_ERR_INVALID, "router_weights: nrouters (%d) must be positive", nrouters);
   const int wpb = 4;
   return launched(launch_pdl(router_weights_kernel, (nrouters + wpb - 1) / wpb, wpb * 32, 0, static_cast<cudaStream_t>(s),
                              logits, mask, nrouters, nexperts, weights),
@@ -288,8 +310,13 @@ extern "C" int ca_router_merge(const void* const* xs, const float* w, int32_t na
   if (nactive < 1 || nactive > kMaxRouterExperts)
     return fail(CA_ERR_INVALID, "router_merge: nactive must be 1..%d (got %d)", kMaxRouterExperts, nactive);
   if (n & 7) return fail(CA_ERR_INVALID, "router_merge: n (%lld) must be a multiple of 8", (long long)n);
+  if (xs == nullptr) return fail(CA_ERR_INVALID, "router_merge: null xs array");
   RouterSources src{};
-  for (int k = 0; k < nactive; ++k) src.p[k] = static_cast<const __nv_bfloat16*>(xs[k]);
+  for (int k = 0; k < nactive; ++k) {
+    if (!aligned(xs[k], 16)) return fail(CA_ERR_INVALID, "router_merge: xs[%d] must be 16-byte aligned", k);
+    src.p[k] = static_cast<const __nv_bfloat16*>(xs[k]);
+  }
+  if (!aligned(y, 16)) return fail(CA_ERR_INVALID, "router_merge: y must be 16-byte aligned");
   return launched(launch_pdl(router_merge_kernel, blocks_for(n / 8, 256), 256, 0, static_cast<cudaStream_t>(s), src, w,
                              nactive, n / 8, static_cast<uint4*>(y)),
                   "router_merge");
@@ -302,6 +329,15 @@ extern "C" int ca_router_merge(const void* const* xs, const float* w, int32_t na
 // internally): eps = u + g*(c-u) in bf16 ops; Euler: x0 = x - bf16(sigma*eps) (0-dim fp32 sigma times a bf16
 // tensor yields bf16), d = (x-x0)/sigma, x' = bf16(x + d*(sigma_next-sigma)); next model input = bf16(x'/div).
 // ---------------------------------------------------------------------------------------------
+// the operands every CFG + scheduler entry point dereferences (model_in_next may be NULL: no next model input)
+static int check_cfg(const char* what, const void* eu, const void* et, const float* lat, long long n, const float* row,
+                     const float* lat_out) {
+  if (n < 0) return fail(CA_ERR_INVALID, "%s: n (%lld) must be >= 0", what, n);
+  if (!eu || !et || !lat) return fail(CA_ERR_INVALID, "%s: null eps_uncond, eps_text or latents_in", what);
+  if (!row) return fail(CA_ERR_INVALID, "%s: null step_row", what);
+  if (!lat_out) return fail(CA_ERR_INVALID, "%s: null latents_out", what);
+  return CA_OK;
+}
 __global__ void cfg_euler_kernel(const __nv_bfloat16* __restrict__ eu, const __nv_bfloat16* __restrict__ et,
                                  const float* __restrict__ lat, long long n, float g, const float* __restrict__ row,
                                  int round_lat, float* __restrict__ lat_out, __nv_bfloat16* __restrict__ next_in) {
@@ -326,6 +362,7 @@ __global__ void cfg_euler_kernel(const __nv_bfloat16* __restrict__ eu, const __n
 }
 extern "C" int ca_cfg_euler(const void* eu, const void* et, const float* lat, int64_t n, float g, const float* step_row,
                             int32_t round_latents_bf16, float* lat_out, void* next_in, void* s) {
+  if (int rc = check_cfg("cfg_euler", eu, et, lat, n, step_row, lat_out)) return rc;
   return launched(launch_pdl(cfg_euler_kernel, blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(s),
                              static_cast<const __nv_bfloat16*>(eu), static_cast<const __nv_bfloat16*>(et), lat, n, g,
                              step_row, round_latents_bf16, lat_out, static_cast<__nv_bfloat16*>(next_in)),
@@ -363,6 +400,8 @@ __global__ void cfg_euler_v_kernel(const __nv_bfloat16* __restrict__ eu, const _
 extern "C" int ca_cfg_euler_v(const void* eu, const void* et, const float* lat, int64_t n, const float* guidance,
                               int32_t frames, int64_t frame_elems, const float* step_row, int32_t round_latents_bf16,
                               float* lat_out, void* next_in, void* s) {
+  if (int rc = check_cfg("cfg_euler_v", eu, et, lat, n, step_row, lat_out)) return rc;
+  if (!guidance) return fail(CA_ERR_INVALID, "cfg_euler_v: null guidance");
   if (frames < 1 || frame_elems < 1 || n % (static_cast<long long>(frames) * frame_elems) != 0)
     return fail(CA_ERR_INVALID, "cfg_euler_v: n (%lld) must be a multiple of frames * frame_elems (%d * %lld)",
                 (long long)n, frames, (long long)frame_elems);
@@ -417,6 +456,7 @@ __global__ void cfg_ddim_kernel(const __nv_bfloat16* __restrict__ eu, const __nv
 }
 extern "C" int ca_cfg_ddim(const void* eu, const void* et, const float* lat, int64_t n, float g, const float* step_row,
                            int32_t round_latents_bf16, int32_t v_prediction, float* lat_out, void* next_in, void* s) {
+  if (int rc = check_cfg("cfg_ddim", eu, et, lat, n, step_row, lat_out)) return rc;
   return launched(launch_pdl(cfg_ddim_kernel, blocks_for(n, 256), 256, 0, static_cast<cudaStream_t>(s),
                              static_cast<const __nv_bfloat16*>(eu), static_cast<const __nv_bfloat16*>(et), lat, n, g,
                              step_row, round_latents_bf16, v_prediction, lat_out, static_cast<__nv_bfloat16*>(next_in)),
@@ -504,6 +544,9 @@ __global__ void i2vgen_latent_encoder_kernel(const __nv_bfloat16* __restrict__ x
 extern "C" int ca_i2vgen_latent_encoder(const void* x, int32_t clips, int32_t frames, int64_t hw, int32_t c_stride,
                                         const float* params, void* y, void* s) {
   if (frames < 1 || frames > 32) return fail(CA_ERR_INVALID, "i2vgen_latent_encoder: frames must be 1..32 (got %d)", frames);
+  if (c_stride < 4) return fail(CA_ERR_INVALID, "i2vgen_latent_encoder: c_stride (%d) must be >= 4", c_stride);
+  if (clips < 1 || hw < 1)
+    return fail(CA_ERR_INVALID, "i2vgen_latent_encoder: clips, hw (%d, %lld) must be positive", clips, (long long)hw);
   const long long total = static_cast<long long>(clips) * hw;
   return launched(launch_pdl(i2vgen_latent_encoder_kernel, static_cast<unsigned>((total + 63) / 64), 64, 0,
                              static_cast<cudaStream_t>(s), static_cast<const __nv_bfloat16*>(x), frames, hw, c_stride,
@@ -574,6 +617,8 @@ extern "C" int ca_frame_conv_small(const void* x, int32_t clips, int32_t frames,
     return fail(CA_ERR_INVALID, "frame_conv_small: cin, cout (%d, %d) must be 1..%d", cin, cout, kFrameConvMaxC);
   if (c_stride < 4 || (c_stride & 3) != 0)
     return fail(CA_ERR_INVALID, "frame_conv_small: c_stride (%d) must be a positive multiple of 4", c_stride);
+  // 8-byte loads of channels 0..3, 4-byte stores of pixel pairs
+  if (!aligned(x, 8) || !aligned(y, 4)) return fail(CA_ERR_INVALID, "frame_conv_small: x must be 8-byte and y 4-byte aligned");
   if (clips < 1 || frames < 1 || hw < 1 || static_cast<long long>(clips) * frames > 65535)
     return fail(CA_ERR_INVALID, "frame_conv_small: clips, frames, hw (%d, %d, %lld) must be positive with clips * frames "
                 "<= 65535", clips, frames, (long long)hw);
@@ -641,6 +686,8 @@ softmax_rows_kernel(const float* __restrict__ x, long long cols, __nv_bfloat16* 
 extern "C" int ca_softmax_rows(const float* x, int64_t rows, int64_t cols, void* y, void* s) {
   if (rows < 1 || rows > 0x7fffffffLL) return fail(CA_ERR_INVALID, "softmax_rows: rows (%lld) must be 1..2^31-1", (long long)rows);
   if (cols < 4 || (cols & 3) != 0) return fail(CA_ERR_INVALID, "softmax_rows: cols (%lld) must be a positive multiple of 4", (long long)cols);
+  // float4 row loads, 8-byte stores of four probabilities
+  if (!aligned(x, 16) || !aligned(y, 8)) return fail(CA_ERR_INVALID, "softmax_rows: x must be 16-byte and y 8-byte aligned");
   return launched(launch_pdl(softmax_rows_kernel, static_cast<unsigned>(rows), 256, 0, static_cast<cudaStream_t>(s), x,
                              cols, static_cast<__nv_bfloat16*>(y)),
                   "softmax_rows");
@@ -709,6 +756,7 @@ extern "C" int ca_vae_latents(const void* moments, const float* noise, int32_t n
                               int32_t layout, int32_t frames, int32_t num_videos, float scale, void* out, void* s) {
   if (moments == nullptr) return fail(CA_ERR_INVALID, "vae_latents: null moments pointer");
   if (out == nullptr) return fail(CA_ERR_INVALID, "vae_latents: null out pointer");
+  if (!aligned(moments, 16)) return fail(CA_ERR_INVALID, "vae_latents: moments must be 16-byte aligned");
   if (latent_channels != 4)
     return fail(CA_ERR_INVALID, "vae_latents: latent_channels (%d) must be 4 (moments carry 8 channels)", latent_channels);
   if (layout < CA_VAE_POSTERIOR || layout > CA_VAE_SVD)

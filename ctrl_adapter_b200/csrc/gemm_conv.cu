@@ -19,9 +19,9 @@ extern "C" int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
   if (geglu && d->n_out * 2 != d->w_rows) return fail(CA_ERR_INVALID, "GEGLU needs w_rows == 2*n_out");
   if (!geglu && d->n_out != d->w_rows) return fail(CA_ERR_INVALID, "n_out must equal w_rows");
   if ((d->n_out & 7) != 0 && !d->out_fp32) return fail(CA_ERR_INVALID, "n_out must be a multiple of 8");
-  if (geglu && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "GEGLU output is bf16");
+  if (geglu && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "GEGLU (act 2) needs out_fp32 = 0: its output is bf16");
   // the fp32 epilogue has no blend term: refuse rather than silently return the unblended result
-  if (d->blend_src && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "AlphaBlender (blend_src) output is bf16");
+  if (d->blend_src && d->out_fp32) return fail(CA_ERR_UNSUPPORTED, "AlphaBlender (blend_src) needs out_fp32 = 0: its output is bf16");
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -43,10 +43,10 @@ extern "C" int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
   for (int t = 0; t < d->ntaps; ++t) max_tap_c = d->tap_c_off[t] > max_tap_c ? d->tap_c_off[t] : max_tap_c;
   int k_per_tap = 0;
   for (int s = 0; s < d->nsrc; ++s) {
-    if (d->a_c_len[s] <= 0 || (d->a_c_off[s] & 7) != 0) return fail(CA_ERR_INVALID, "bad channel slice");
+    if (d->a_c_len[s] <= 0 || (d->a_c_off[s] & 7) != 0) return fail(CA_ERR_INVALID, "a_c_len of source %d must be positive and a_c_off a multiple of 8", s);
     if (s == 0 && d->nsrc == 2 && (d->a_c_len[0] % 64) != 0)
       return fail(CA_ERR_INVALID, "first of two sources must contribute a multiple of 64 channels");
-    if (max_tap_c + d->a_c_off[s] + d->a_c_len[s] > d->a_channels[s]) return fail(CA_ERR_INVALID, "channel slice exceeds tensor");
+    if (max_tap_c + d->a_c_off[s] + d->a_c_len[s] > d->a_channels[s]) return fail(CA_ERR_INVALID, "a_c_off + a_c_len (+ tap_c_off) of source %d exceeds a_channels", s);
     p.src_c[s] = d->a_c_len[s];
     p.src_c0_off[s] = d->a_c_off[s];
     k_per_tap += d->a_c_len[s];

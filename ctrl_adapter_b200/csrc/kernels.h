@@ -20,6 +20,10 @@ int launched(cudaError_t e, const char* what);
 int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
               const cuuint32_t* box);
 int num_sms();
+// argument checks: a pointer the kernel accesses in `bytes`-wide vectors (a null pointer passes), and the largest
+// gridDim.y / gridDim.z a launch may have
+inline bool aligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1u)) == 0; }
+constexpr long long kMaxGridYZ = 65535;
 
 // --- gemm_conv.cu / gemm_conv_bn*.cu ---
 struct GemmParams {

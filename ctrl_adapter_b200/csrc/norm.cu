@@ -99,10 +99,18 @@ static int check_gn_channels(const char* what, int c0, int c1, int groups) {
     return fail(CA_ERR_INVALID, "%s: c0, c1 (%d, %d) must be multiples of 8 with 8 <= c0 + c1 <= 4096", what, c0, c1);
   return CA_OK;
 }
+// both passes: n is gridDim.y; the sources are read in 16-byte vectors
+static int check_gn_sources(const char* what, const void* x0, const void* x1, int c1, int n) {
+  if (n < 1 || n > kMaxGridYZ) return fail(CA_ERR_INVALID, "%s: n (%d) must be 1..65535", what, n);
+  if (!aligned(x0, 16) || (c1 > 0 && !aligned(x1, 16))) return fail(CA_ERR_INVALID, "%s: x0, x1 must be 16-byte aligned", what);
+  return CA_OK;
+}
 
 extern "C" int ca_groupnorm_stats(const void* x0, int32_t c0, const void* x1, int32_t c1, int32_t n, int64_t rows,
                                   int32_t groups, double* sums, void* s) {
   if (int rc = check_gn_channels("groupnorm_stats", c0, c1, groups)) return rc;
+  if (int rc = check_gn_sources("groupnorm_stats", x0, x1, c1, n)) return rc;
+  if (rows < 1) return fail(CA_ERR_INVALID, "groupnorm_stats: rows (%lld) must be positive", (long long)rows);
   cudaStream_t stream = static_cast<cudaStream_t>(s);
   cudaError_t e = cudaMemsetAsync(sums, 0, sizeof(double) * n * groups * 2, stream);
   if (e != cudaSuccess) return launched(e, "groupnorm_stats");
@@ -230,6 +238,12 @@ extern "C" int ca_groupnorm_apply(const void* x0, int32_t c0, const void* x1, in
                                   int32_t w, int32_t imgs_per_sample, int32_t groups, float eps, const double* sums,
                                   const float* gamma, const float* beta, int32_t silu, int32_t up2x, void* y, void* s) {
   if (int rc = check_gn_channels("groupnorm_apply", c0, c1, groups)) return rc;
+  if (int rc = check_gn_sources("groupnorm_apply", x0, x1, c1, n)) return rc;
+  if (!aligned(y, 16)) return fail(CA_ERR_INVALID, "groupnorm_apply: y must be 16-byte aligned");
+  if (h < 1 || w < 1) return fail(CA_ERR_INVALID, "groupnorm_apply: h, w (%d, %d) must be positive", h, w);
+  // image i reads the statistics of sample i / imgs_per_sample: a partial last sample would read past them
+  if (imgs_per_sample < 1 || n % imgs_per_sample != 0)
+    return fail(CA_ERR_INVALID, "groupnorm_apply: imgs_per_sample (%d) must be positive and divide n (%d)", imgs_per_sample, n);
   const long long hw = static_cast<long long>(h) * w;
   if (hw > 0x3fffffffLL) return fail(CA_ERR_INVALID, "groupnorm_apply: h * w (%lld) must be < 2^30", hw);
   const int C = c0 + c1;
@@ -476,6 +490,11 @@ extern "C" int ca_layernorm(const void* x_, int64_t rows, int32_t c, float eps, 
     return fail(CA_ERR_INVALID, "layernorm: c (%d) must be a multiple of 8 in 8..%d", c, kLnMaxC);
   // whole rows travel as 1-D bulk copies
   if ((reinterpret_cast<uintptr_t>(x_) & 15) != 0) return fail(CA_ERR_INVALID, "layernorm: x must be 16-byte aligned");
+  // float4 loads of gamma / beta, 16-byte loads of the row vector and 16-byte stores of y / y_sum
+  if (!aligned(gamma, 16) || !aligned(beta, 16))
+    return fail(CA_ERR_INVALID, "layernorm: gamma, beta must be 16-byte aligned");
+  if (!aligned(add_rowvec_, 16) || !aligned(y_sum_, 16) || !aligned(y_, 16))
+    return fail(CA_ERR_INVALID, "layernorm: add_rowvec, y_sum, y must be 16-byte aligned");
   if (rows <= 0) return CA_OK;
   if (rows >= (1LL << 31) - 64) return fail(CA_ERR_INVALID, "layernorm: rows (%lld) must be < 2^31 - 64", (long long)rows);
   const auto* x = static_cast<const __nv_bfloat16*>(x_);

@@ -167,6 +167,7 @@ extern "C" int ca_temporal_attention(const void* q, const void* k, const void* v
   if (frames < 1 || frames > 32) return fail(CA_ERR_INVALID, "temporal_attention: frames must be 1..32 (got %d)", frames);
   if (clips < 1 || hw < 1 || heads < 1) return fail(CA_ERR_INVALID, "temporal_attention: empty problem (clips, hw, heads)");
   if ((in_row_stride & 7) != 0) return fail(CA_ERR_INVALID, "temporal_attention: in_row_stride must be a multiple of 8");
+  if (!aligned(out, 4)) return fail(CA_ERR_INVALID, "temporal_attention: out must be 4-byte aligned");
   // one CTA per (clip, group of 128 / SEQ pixels, head)
   const int seq = frames <= 16 ? 16 : 32;
   const long long ctas = static_cast<long long>(clips) * ((hw + 128 / seq - 1) / (128 / seq)) * heads;

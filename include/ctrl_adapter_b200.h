@@ -32,7 +32,7 @@ enum ca_act { CA_ACT_NONE = 0, CA_ACT_SILU = 1, CA_ACT_GEGLU = 2 };
 int ca_abi_version(void);
 /* Thread-local description of the last non-zero status returned on this thread. */
 const char* ca_last_error(void);
-/* 0 when a CUDA device with compute capability 10.x is usable by this process, else non-zero. */
+/* 0 when a CUDA device with compute capability 9.x (sm_90a) is usable by this process, else non-zero. */
 int ca_device_ok(void);
 
 /*
@@ -80,7 +80,9 @@ typedef struct ca_gemm_desc {
   int64_t out_strides[4];    /* element strides of the output rows */
   /* epilogue, applied in this order with a bf16 rounding after every step (autocast rounding points):
    *   v = acc + bias ; v = act(v) ; v *= out_scale ; v += rowvec ; v += residual ;
-   *   v = alpha * blend_src + (1 - alpha) * v                                            */
+   *   v = alpha * blend_src + (1 - alpha) * v
+   * out_fp32 = 1 rounds to bf16 only after act (SiLU) and after the rowvec add; bias, out_scale and the residual add
+   * stay fp32; there is no GEGLU and no blend term (CA_ERR_UNSUPPORTED).                  */
   int32_t act;
   float out_scale;
   const void* rowvec;        /* bf16, addressed rowvec[sum_d o_d * rowvec_strides[d] + n] */
@@ -99,7 +101,8 @@ int ca_gemm(const ca_gemm_desc* d, void* cuda_stream);
  * model/adapter_spatial_temporal.py:271 (adapter spatial self / cross attention), the ControlNet
  * Transformer2DModel blocks built at controlnet/controlnet.py:371-424 and the UNet attention layers.
  * q/k/v: [batch, L, heads * head_dim_pad] bf16 with head_dim_pad a multiple of 64 (zero padded),
- * row strides given in elements.  out: [batch, lq, heads * head_dim_pad].
+ * row strides given in elements.  out: [batch, lq, heads * head_dim_pad], 4-byte aligned, even out strides.
+ * Constraints: batch <= 65535, heads * head_dim_pad / 64 <= 65535.
  */
 typedef struct ca_attention_desc {
   const void* q; const void* k; const void* v; void* out;
@@ -122,6 +125,9 @@ int ca_attention(const ca_attention_desc* d, void* cuda_stream);
  * model/adapter_spatial_temporal.py:254, diffusers TemporalResnetBlock / Transformer2DModel norms.
  * `sums` is a caller-provided scratch of n*groups*2 doubles (zeroed by ca_groupnorm_stats).
  * A "sample" is `rows` consecutive channel vectors (h*w, or frames*h*w for the 5-D temporal GroupNorm).
+ * Constraints (both passes): 1 <= groups <= 64 dividing c0 + c1; c0, c1 multiples of 8 with 8 <= c0 + c1 <= 4096;
+ * 1 <= n <= 65535; x0 (and x1 when c1 > 0) and y 16-byte aligned; stats: rows >= 1; apply: h, w >= 1, h * w < 2^30,
+ * imgs_per_sample >= 1 dividing n (apply's n counts images, stats' n samples).
  */
 int ca_groupnorm_stats(const void* x0, int32_t c0, const void* x1, int32_t c1, int32_t n, int64_t rows,
                        int32_t groups, double* sums, void* cuda_stream);
@@ -135,50 +141,60 @@ int ca_groupnorm_apply(const void* x0, int32_t c0, const void* x1, int32_t c1, i
  * Replaces F.layer_norm in diffusers BasicTransformerBlock / TemporalBasicTransformerBlock (norm1/2/3, norm_in)
  * and the `hidden_states + emb` add at model/adapter_spatial_temporal.py:279.
  * Constraints: c a multiple of 8, 8 <= c <= 2048; x contiguous [rows, c] and 16-byte aligned (whole rows travel as
- * 1-D bulk copies); rows < 2^31.  y / y_sum may alias x (each row is read before it is written).
+ * 1-D bulk copies); gamma, beta, add_rowvec, y_sum and y 16-byte aligned; rows < 2^31 - 64.  y / y_sum may alias x
+ * (each row is read before it is written).
  */
 int ca_layernorm(const void* x, int64_t rows, int32_t c, float eps, const float* gamma, const float* beta,
                  const void* add_rowvec, int64_t rows_per_vec, void* y_sum, void* y, void* cuda_stream);
 
 /* Sinusoidal timestep embedding (diffusers Timesteps; model/adapter_spatial_temporal.py:207,263;
  * controlnet/controlnet.py:751).  t: n fp32 device values.  round_t_bf16 reproduces the reference's
- * `timestep.to(bf16)` before the sinusoid (adapter_spatial_temporal.py:198).  out: [n, dim] bf16. */
+ * `timestep.to(bf16)` before the sinusoid (adapter_spatial_temporal.py:198).  out: [n, dim] bf16; an odd dim ends in
+ * a zero column.  Constraints: n >= 1, dim >= 2. */
 int ca_timestep_embedding(const float* t, int32_t n, int32_t dim, int32_t flip_sin_to_cos, float freq_shift,
                           int32_t round_t_bf16, void* out, void* cuda_stream);
 
-/* Elementwise helpers (bf16 in/out). */
+/* Elementwise helpers (bf16 in/out): n a multiple of 8, every pointer 16-byte aligned. */
 int ca_silu(const void* x, int64_t n, void* y, void* cuda_stream);
 int ca_add(const void* a, const void* b, int64_t n, void* y, void* cuda_stream);
-/* NCHW (bf16 or fp32) -> channels-last bf16 with the channel count zero padded to c_pad, and back. */
+/* NCHW (bf16 or fp32) -> channels-last bf16 with the channel count zero padded to c_pad, and back (the first c of
+ * c_stride channels).  Constraints: n, c, hw >= 1; c <= c_pad (c <= c_stride); n <= 65535; c_pad (c) <= 65535 * 32;
+ * hw < 2^32. */
 int ca_nchw_to_nhwc(const void* x, int32_t src_fp32, int32_t n, int32_t c, int64_t hw, int32_t c_pad, void* y,
                     void* cuda_stream);
 int ca_nhwc_to_nchw(const void* x, int32_t n, int32_t c, int32_t c_stride, int64_t hw, void* y, int32_t dst_fp32,
                     void* cuda_stream);
-/* F.adaptive_avg_pool2d for integer ratios (sdxl pipeline :1308-1309), channels-last. */
+/* F.adaptive_avg_pool2d for integer ratios (sdxl pipeline :1308-1309), channels-last: oh, ow >= 1 dividing h, w. */
 int ca_avgpool(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, int32_t oh, int32_t ow, void* y,
                void* cuda_stream);
-/* nearest 2x up-sampling, channels-last (diffusers Upsample2D in the UNet up blocks). */
+/* nearest 2x up-sampling, channels-last (diffusers Upsample2D in the UNet up blocks): c a multiple of 8, x and y
+ * 16-byte aligned. */
 int ca_upsample2x(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, void* y, void* cuda_stream);
 
 /*
  * Router (model/ctrl_router.py:85-112): masked softmax over experts for all routers in one launch,
  * one warp per router (warp-shuffle reduction).  logits [nrouters, nexperts] fp32, mask [nexperts] (0 = masked).
+ * Constraints: nrouters >= 1, 1 <= nexperts <= 32.
  */
 int ca_router_weights(const float* logits, const uint8_t* mask, int32_t nrouters, int32_t nexperts, float* weights,
                       void* cuda_stream);
 /* Row softmax, fp32 [rows, cols] -> bf16 probabilities (cols % 4 == 0): the VAE decoder's single 512-wide attention
  * head (diffusers AutoencoderKL mid block, reached from sdxl pipeline :1414 / i2vgen pipeline :398-418) runs as
- * GEMM (QK^T, fp32) -> this -> GEMM (PV).  softmax in fp32, one rounding to bf16 (torch SDPA math semantics). */
+ * GEMM (QK^T, fp32) -> this -> GEMM (PV).  softmax in fp32, one rounding to bf16 (torch SDPA math semantics).  x 16-byte, y 8-byte aligned;
+ * 1 <= rows < 2^31. */
 int ca_softmax_rows(const float* x, int64_t rows, int64_t cols, void* y, void* cuda_stream);
 /* Conv3d (3,1,1), padding (1,0,0) over the frame axis for <= 4 channels: time_conv_out of the SVD VAE's TemporalDecoder
  * (diffusers AutoencoderKLTemporalDecoder, run by the svd pipeline's decode_latents :265-292).  x: channels-last bf16
  * [clips*frames, hw, c_stride] (the first cin channels are read); w / bias: HOST arrays [cout][cin][3] / [cout] (they
- * travel to the kernel by value, so the call is CUDA-graph capturable); y: bf16 [clips*frames, cout, hw] (logical NCHW). */
+ * travel to the kernel by value, so the call is CUDA-graph capturable); y: bf16 [clips*frames, cout, hw] (logical NCHW).
+ * Constraints: 1 <= cin, cout <= 4; c_stride a positive multiple of 4; clips * frames <= 65535; x 8-byte and y 4-byte
+ * aligned. */
 int ca_frame_conv_small(const void* x, int32_t clips, int32_t frames, int64_t hw, int32_t c_stride, int32_t cin,
                         int32_t cout, const float* w_host, const float* bias_host, void* y, void* cuda_stream);
 /* Weighted merge of expert residuals (i2vgen_xl pipeline :1001-1022): y = sum_e w[e] * xs[e], bf16 rounding
  * after each multiply and each add as in the reference loop.  xs: HOST array of nactive (<= 8) device pointers; they
- * travel to the kernel by value, so the call is CUDA-graph capturable. */
+ * travel to the kernel by value, so the call is CUDA-graph capturable.  n a multiple of 8; every xs[k] and y 16-byte
+ * aligned. */
 int ca_router_merge(const void* const* xs, const float* w, int32_t nactive, int64_t n, void* y, void* cuda_stream);
 
 /* Classifier-free guidance + scheduler update in one pass (latent-sized, HBM-bound).
@@ -188,14 +204,16 @@ int ca_router_merge(const void* const* xs, const float* w, int32_t nactive, int6
  *   eps = u + g (c - u); x0 = x - sigma*eps; d = (x - x0)/sigma; x' = x + d (sigma_next - sigma);
  *   also emits the next step's scaled model input x' / sqrt(sigma_next^2+1) in bf16 (scale_model_input, :1285).
  * DDIM = I2VGen-XL (i2vgen_xl pipeline :1102-1115), eta = 0, epsilon prediction.
- * round_latents_bf16 = 1 reproduces the reference's bf16 latents between steps. */
+ * round_latents_bf16 = 1 reproduces the reference's bf16 latents between steps.  All three: n >= 0; eps_uncond, eps_text,
+ * latents_in, step_row and latents_out non-NULL (model_in_next may be NULL: no next model input). */
 int ca_cfg_euler(const void* eps_uncond, const void* eps_text, const float* latents_in, int64_t n, float guidance,
                  const float* step_row, int32_t round_latents_bf16, float* latents_out, void* model_in_next,
                  void* cuda_stream);
 /* Euler, v-prediction, per-frame guidance = the SVD loop (svd pipeline :781-787; EulerDiscreteScheduler with
  * prediction_type v_prediction): latents [clips, frames, C, H, W], guidance: DEVICE fp32 [frames] (bf16-valued, the
  * pipeline's linspace(min, max, F) in the latent dtype), frame_elems = C*H*W.  step_row as for ca_cfg_euler.
- *   mo = u + g_f (c - u);  x0 = mo * (-sigma / sqrt(sigma^2+1)) + x / (sigma^2+1);  x' = x + (x - x0)/sigma * (sigma_next - sigma) */
+ *   mo = u + g_f (c - u);  x0 = mo * (-sigma / sqrt(sigma^2+1)) + x / (sigma^2+1);  x' = x + (x - x0)/sigma * (sigma_next - sigma)
+ * frames, frame_elems >= 1, n a multiple of frames * frame_elems, guidance non-NULL. */
 int ca_cfg_euler_v(const void* eps_uncond, const void* eps_text, const float* latents_in, int64_t n,
                    const float* guidance, int32_t frames, int64_t frame_elems, const float* step_row,
                    int32_t round_latents_bf16, float* latents_out, void* model_in_next, void* cuda_stream);
@@ -206,7 +224,8 @@ int ca_cfg_ddim(const void* eps_uncond, const void* eps_text, const float* laten
 /* I2VGen-XL image-latent temporal encoder (unet_i2vgen_xl.py:51-101, called at :648): per pixel, over the F frames of a
  * clip, on 4 channels: h = x + to_out(attn(LN(x))) (2 heads x 4); y = h + W2 gelu(W1 h).  Step-invariant conditioning,
  * computed once per generation.  x/y: [clips*frames, hw, c_stride] bf16 (first 4 channels used).  params: fp32 device
- * array {ln_w[4], ln_b[4], wq[8*4], wk[8*4], wv[8*4], wo[4*8], bo[4], w1[16*4], b1[16], w2[4*16], b2[4]}. */
+ * array {ln_w[4], ln_b[4], wq[8*4], wk[8*4], wv[8*4], wo[4*8], bo[4], w1[16*4], b1[16], w2[4*16], b2[4]}.
+ * Constraints: 1 <= frames <= 32, c_stride >= 4, clips, hw >= 1. */
 int ca_i2vgen_latent_encoder(const void* x, int32_t clips, int32_t frames, int64_t hw, int32_t c_stride,
                              const float* params, void* y, void* cuda_stream);
 
@@ -222,7 +241,7 @@ int ca_i2vgen_latent_encoder(const void* x, int32_t clips, int32_t frames, int64
  *                                            nv times, then twice for classifier-free guidance (i2vgen pipeline :487-517)
  *   CA_VAE_SVD        [2*n*nv, frames, 4, hw] cat([zeros, v]) repeated nv times, then repeated over the frames
  *                                            (svd pipeline :214-235, :580-583)
- * latent_channels must be 4.
+ * latent_channels must be 4; moments 16-byte aligned.
  */
 enum ca_vae_layout { CA_VAE_POSTERIOR = 0, CA_VAE_I2VGEN = 1, CA_VAE_SVD = 2 };
 int ca_vae_latents(const void* moments, const float* noise, int32_t n, int64_t hw, int32_t latent_channels,
@@ -233,6 +252,7 @@ int ca_vae_latents(const void* moments, const float* noise, int32_t n, int64_t h
  * model/adapter_spatial_temporal.py:280).  q/k/v: rows of heads*64 bf16 with stride in_row_stride elements (views of a
  * fused QKV buffer), out: [clips*frames*hw, heads*64] dense; rows in (clip, frame, pixel)
  * order -- the (b f) s c <-> (b s) f c permutes of the reference are folded into the addressing.
+ * Constraints: 1 <= frames <= 32; in_row_stride a multiple of 8; out 4-byte aligned.
  */
 int ca_temporal_attention(const void* q, const void* k, const void* v, int32_t clips, int32_t frames, int64_t hw,
                           int32_t heads, float scale, int64_t in_row_stride, void* out, void* cuda_stream);

@@ -661,6 +661,27 @@ def _epilogue_chain64(v, *, act=0, scale=1.0, rv=None, res=None, xs=None, alpha=
     return v, 2 ** -6 if multi else 2 ** -7, mag if (multi or xs is not None) else None
 
 
+def _f32_epilogue_verdict(name, pre, out, a, rv, dims, rows=None):
+    """the fp32-output epilogue applied in float64 to the kernel's own fp32 pre-activation (bias included): SiLU rounded
+    to bf16, x out_scale, + row vector rounded to bf16, + residual NOT rounded (include/ctrl_adapter_b200.h).  A rounding
+    step may flip one bf16 ulp of its intermediate (rtol 2^-7 of the largest one); without one the tolerance is a few
+    fp32 ulps of the largest intermediate, so a rounded residual sum (half a bf16 ulp) fails."""
+    v = pre.to(F64)
+    rounded = a["act"] == 1 or rv is not None
+    if a["act"] == 1:
+        v = _r64(F.silu(v))
+    if a["out_scale"] != 1.0:
+        v = v * a["out_scale"]
+    mag = v.abs()
+    if rv is not None:
+        v = _r64(v + rv)
+        mag = torch.maximum(mag, v.abs())
+    if a["residual"] is not None:
+        v = v + a["residual"].to(F64)
+        mag = torch.maximum(mag, v.abs())
+    return _report(name, out, v, 2 ** -7 if rounded else 2 ** -20, 1e-6, mag=mag, dims=dims, rows=rows)
+
+
 def _sum_floor(abs_sum):
     """absolute floor of the fp32-accumulation checks: atol 1e-4, raised to 2^-16 of sum |x_k w_k| where that is larger.
     Where the products cancel, an fp32 sum over K terms is off by a multiple of 2^-24 of sum |x_k w_k| that grows with
@@ -677,7 +698,8 @@ _PRE_ONLY = dict(act=0, out_scale=1.0, rowvec=None, residual=None, blend_src=Non
 
 
 def linear_verdict(name, a, out, rerun):
-    """ops.linear.  fp32 output: the float64 product (x out_scale, + residual) at rtol 1e-3 / atol 1e-4.  bf16 output:
+    """ops.linear.  fp32 output: the float64 product (x out_scale) at rtol 1e-3 / atol 1e-4; with SiLU, a row vector or
+    a residual, the pre-activation at that tolerance and then _f32_epilogue_verdict on it.  bf16 output:
     rerun(**changes) -- the same call with fp32 output and only the bias (same kernel, tiles and summation order) -- vs
     float64 at that tolerance, then the epilogue's rounding chain applied in float64 to that pre-activation.  A
     pre-activation within an fp32 ulp or two of a bf16 rounding tie rounds either way depending on the summation order
@@ -690,13 +712,19 @@ def linear_verdict(name, a, out, rerun):
     if bias is not None:
         exact = exact + bias.to(F64)
     dims = ("row", "col")
+    rv = a["rowvec"]
+    if rv is not None:
+        rv = rv.to(F64).repeat_interleave(a["rows_per_vec"], dim=0)
     if a["out_fp32"]:
-        if act != 0 or a["rowvec"] is not None or a["blend_src"] is not None:
-            raise NotImplementedError("linear: fp32 output with an activation, row vector or blend")
-        ref = exact * a["out_scale"] if a["out_scale"] != 1.0 else exact
-        if a["residual"] is not None:
-            ref = ref + a["residual"].to(F64)
-        return [_report(name, out, ref, 1e-3, atol * abs(a["out_scale"]), dims=dims)]
+        if act == 2 or a["blend_src"] is not None:
+            raise NotImplementedError("linear: fp32 output with GEGLU or blend")
+        if act == 0 and rv is None and a["residual"] is None:
+            ref = exact * a["out_scale"] if a["out_scale"] != 1.0 else exact
+            return [_report(name, out, ref, 1e-3, atol * abs(a["out_scale"]), dims=dims)]
+        pre = rerun(**_PRE_ONLY)
+        _sync()
+        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims),
+                _f32_epilogue_verdict(name, pre, out, a, rv, dims)]
     pre = rerun(**_PRE_ONLY)
     _sync()
     recs = [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims)]
@@ -708,11 +736,10 @@ def linear_verdict(name, a, out, rerun):
         h = _r64(torch.cat([p4[:, :, 0].reshape(m, n), p4[:, :, 1].reshape(m, n)], dim=1))
         recs.append(_report(name, out, _r64(h[:, :n] * _r64(F.gelu(h[:, n:]))), 2 ** -6, 2e-3, dims=dims))
         return recs
-    rv = a["rowvec"]
     f64 = (lambda t: None if t is None else t.to(F64))
     ref, rtol, mag = _epilogue_chain64(
         pre.to(F64), act=act, scale=a["out_scale"], res=f64(a["residual"]), xs=f64(a["blend_src"]),
-        alpha=a["blend_alpha"], rv=None if rv is None else rv.to(F64).repeat_interleave(a["rows_per_vec"], dim=0))
+        alpha=a["blend_alpha"], rv=rv)
     recs.append(_report(name, out, ref, rtol, 1e-3, mag=mag, dims=dims))
     return recs
 
@@ -744,9 +771,19 @@ def conv2d_verdict(name, a, out, rerun, rows=None):
     del xd
     dims = ("img", "y", "x", "ch")
     f64 = (lambda t: None if t is None else t[ii].to(F64))
+    if a["out_fp32"] and (a["act"] != 0 or a["rowvec"] is not None or a["residual"] is not None):
+        if a["blend_src"] is not None:
+            raise NotImplementedError("conv2d: fp32 output with a blend")
+        pre = rerun(**_PRE_ONLY)[ii]
+        _sync()
+        rv = a["rowvec"]
+        if rv is not None:
+            rv = (rv[ii] if rv.shape[0] > 1 else rv).to(F64)[:, None, None, :]
+        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims, rows=rows),
+                _f32_epilogue_verdict(name, pre, out[ii], {**a, "residual": f64(a["residual"])}, rv, dims, rows)]
     if a["out_fp32"]:
-        if a["act"] != 0 or a["rowvec"] is not None or a["blend_src"] is not None:
-            raise NotImplementedError("conv2d: fp32 output with an activation, row vector or blend")
+        if a["blend_src"] is not None:
+            raise NotImplementedError("conv2d: fp32 output with a blend")
         ref = exact * a["out_scale"] if a["out_scale"] != 1.0 else exact
         if a["residual"] is not None:
             ref = ref + f64(a["residual"])

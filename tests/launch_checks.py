@@ -5,14 +5,16 @@ modules call `ops.X` through the module, so replacing the attribute is enough, a
 call is keyed by its configuration: the op; shape, strides, dtype, 16-byte alignment and aliasing of every tensor
 argument; every scalar argument.  The first call with a key:
   1. clones its inputs, keeping strides, alignment and aliasing (views of a wider buffer stay views of a buffer of the
-     same width);
+     same width), into buffers with 256-byte guard bands; bytes outside the views are NaN for floating-point inputs
+     and a fixed pattern otherwise;
   2. runs the real kernel and synchronises;
   3. checks what it wrote against the op's reference (VERIFIERS: the per-launch verdicts of tests/kernel_checks.py, so
      the layout checks and the census share one reference per op) and, for an `out=` view, that the bytes around it in
      its buffer are unchanged;
   4. replays the call on the clones -- into NaN-filled outputs where the op takes them -- and requires the replay to be
-     bit-identical to the in-step output; group_norm, whose statistics are summed with float atomics, must pass its
-     reference again instead.
+     bit-identical to the in-step output (a read of a guard band or stride gap picks up NaN there); group_norm, whose
+     statistics are summed with float atomics, must pass its reference again instead; and every byte outside the
+     argument views must keep its fill.
 Later calls with the same key are only counted.  A call without a verifier, or one its verifier cannot handle, fails.
 Where the float64 reference of a whole launch would be too large, it is evaluated on the first, middle and last image /
 batch entry / sample (never on part of an image) and the row says so.
@@ -121,6 +123,7 @@ def _v_timestep_embedding(a, out, rerun):
     freq = torch.exp(-math.log(10000.0) * torch.arange(half, device=t.device, dtype=F64) / (half - a["freq_shift"]))
     arg = t[:, None] * freq[None, :]
     ref = torch.cat([torch.cos(arg), torch.sin(arg)] if a["flip_sin_to_cos"] else [torch.sin(arg), torch.cos(arg)], -1)
+    ref = F.pad(ref, (0, dim - 2 * half))  # odd dim: a trailing zero column
     return [kc._report("timestep_embedding", out, kc._r64(ref), 2 ** -7, 4e-3, dims=("t", "ch"))], False
 
 
@@ -245,30 +248,67 @@ def _bytes(storage, device, lo, hi):
     return torch.empty(0, dtype=torch.uint8, device=device).set_(storage, lo, (hi - lo,))
 
 
+GUARD = 256          # bytes of guard band before and after every cloned buffer
+NAN_BYTE = 0xFF      # 0xFFFF / 0xFFFFFFFF: NaN in bf16, fp32 and fp64
+PATTERN_BYTE = 0xA5  # outputs and integer inputs
+
+
+def _view_on(storage, t, byte_off):
+    return torch.empty(0, dtype=t.dtype, device=t.device).set_(storage, byte_off // t.element_size(), t.shape, t.stride())
+
+
+def _dense(views, lo, hi):
+    """the contiguous views among `views` cover the byte range [lo, hi) with no gap"""
+    spans = sorted(_byte_range(t) for t in views if t.is_contiguous())
+    end = lo
+    for a, b in spans:
+        if a > end:
+            return False
+        end = max(end, b)
+    return end >= hi
+
+
 class _Clone:
     """copies of the argument tensors: per storage, one buffer holding the byte range the call's views of it cover, at
-    the same address modulo 16; every view re-created on it with its own shape and strides"""
+    the same address modulo 16, with GUARD bytes before and after it; every view re-created on it with its own shape
+    and strides.  Only the views' elements are copied: every other byte -- guard bands and stride gaps -- is NaN where
+    the buffer holds a floating-point input and PATTERN_BYTE otherwise, so a kernel that reads outside its operands
+    gets NaN (or garbage) instead of the caching allocator's leftovers, and a stray write shows up as a changed byte.
+    Views that share a storage (a fused QKV buffer, an output aliasing an input) share the buffer, so they keep their
+    real neighbours."""
 
     def __init__(self, args):
-        self.groups = {}
-        for _, t in _flat_tensors(args):
+        self.groups, self.orig, self.views, self.fill = {}, {}, {}, {}
+        for label, t in _flat_tensors(args):
             lo, hi = _byte_range(t)
-            g = self.groups.setdefault(_storage_key(t), [t.untyped_storage(), lo, hi])
+            key = _storage_key(t)
+            g = self.groups.setdefault(key, [t.untyped_storage(), lo, hi])
             g[1], g[2] = min(g[1], lo), max(g[2], hi)
-        self.bufs = {}
+            self.views.setdefault(key, []).append(t)
+            if t.is_floating_point() and label.split("[")[0] not in OUT_ARGS:
+                self.fill[key] = NAN_BYTE
+            if label in OUT_ARGS:
+                self.orig[key] = None
+        self.bufs, self.dense = {}, {}
         for key, (st, lo, hi) in self.groups.items():
-            buf = torch.empty(hi - lo + 16, dtype=torch.uint8, device=key[0])
-            shift = (st.data_ptr() + lo - buf.data_ptr()) % 16
-            buf[shift:shift + hi - lo].copy_(_bytes(st, key[0], lo, hi))
+            self.dense[key] = _dense(self.views[key], lo, hi)
+            if key in self.orig and not _dense([t for t in self.views[key] if t.is_contiguous()
+                                                and _byte_range(t) == (lo, hi)], lo, hi):
+                # an out= view with bytes around it in its storage: what untouched_around compares with
+                self.orig[key] = _bytes(st, key[0], lo, hi).clone()
+            buf = torch.full((hi - lo + 2 * GUARD + 16,), self.fill.get(key, PATTERN_BYTE), dtype=torch.uint8,
+                             device=key[0])
+            shift = GUARD + (st.data_ptr() + lo - buf.data_ptr()) % 16
             self.bufs[key] = (buf, shift)
+            for t in self.views[key]:
+                self.view(t).copy_(t)
 
     def view(self, t):
         buf, shift = self.bufs[_storage_key(t)]
         lo = self.groups[_storage_key(t)][1]
         off = shift + t.storage_offset() * t.element_size() - lo
         assert off % t.element_size() == 0
-        return torch.empty(0, dtype=t.dtype, device=t.device).set_(
-            buf.untyped_storage(), off // t.element_size(), t.shape, t.stride())
+        return _view_on(buf.untyped_storage(), t, off)
 
     def args(self, args):
         out = {}
@@ -285,15 +325,35 @@ class _Clone:
         """the bytes of t's buffer range outside the views in `written` are what they were before the call"""
         key = _storage_key(t)
         st, lo, hi = self.groups[key]
-        buf, shift = self.bufs[key]
+        if self.orig[key] is None:  # the view is its storage's whole range: there is nothing around it
+            return True
         now = _bytes(st, key[0], lo, hi).clone()
         for w in written:  # put the pre-call values back where the call was allowed to write
             if _storage_key(w) == key:
                 es = w.element_size()
-                dst = torch.empty(0, dtype=w.dtype, device=w.device).set_(
-                    now.untyped_storage(), (w.storage_offset() * es - lo) // es, w.shape, w.stride())
-                dst.copy_(self.view(w))
-        return torch.equal(now, buf[shift:shift + hi - lo])
+                _view_on(now.untyped_storage(), w, w.storage_offset() * es - lo).copy_(self.view(w))
+        return torch.equal(now, self.orig[key])
+
+    def stray_bytes(self):
+        """labels of the buffers where a byte that belongs to no argument view lost its fill (guard band or gap)"""
+        bad = []
+        for key, (buf, shift) in self.bufs.items():
+            lo, hi = self.groups[key][1:]
+            fill = self.fill.get(key, PATTERN_BYTE)
+            if self.dense[key]:  # the views tile the range: only the guard bands are outside them
+                if not (bool((buf[:shift] == fill).all()) and bool((buf[shift + hi - lo:] == fill).all())):
+                    bad.append(key)
+                continue
+            covered = torch.zeros_like(buf)
+            for t in self.views[key]:
+                m = _bits(_view_on(covered.untyped_storage(), t, shift + t.storage_offset() * t.element_size() - lo))
+                m.fill_(255 if m.dtype == torch.uint8 else -1)
+            step = 1 << 26  # bounded temporaries: the buffers of a production launch reach gigabytes
+            if any(bool(((buf[i:i + step] != fill) & (covered[i:i + step] == 0)).any())
+                   for i in range(0, buf.numel(), step)):
+                bad.append(key)
+            del covered
+        return bad
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -452,6 +512,8 @@ class Recorder:
                 outs2 = _tensor_outputs(ret2, rp)
                 if len(outs2) != len(outs) or not all(_same_bits(x, y) for x, y in zip(outs, outs2)):
                     row.fail("replay not bit-identical to the in-step launch")
+            if clone.stray_bytes():
+                row.fail("replay wrote into a guard band or a stride gap of an argument buffer")
         except Exception as e:  # a launch its verifier cannot handle fails its row
             row.fail(f"{type(e).__name__}: {e}"[:300])
         return ret

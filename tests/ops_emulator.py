@@ -27,8 +27,12 @@ def _r(x: torch.Tensor) -> torch.Tensor:
 
 def _epilogue(acc, bias, act, out_scale, rowvec, residual, blend_src, blend_alpha, out_fp32):
     v = acc if bias is None else acc + bias.float()
-    if out_fp32:
+    if out_fp32:  # rounded to bf16 only after SiLU and after the row vector
+        if act == ACT_SILU:
+            v = _r(F.silu(v))
         v = v * out_scale if out_scale != 1.0 else v
+        if rowvec is not None:
+            v = _r(v + rowvec.float())
         return v if residual is None else v + residual.float()
     v = _r(v)
     if act == ACT_SILU:
@@ -185,7 +189,7 @@ def timestep_embedding(t, dim, *, flip_sin_to_cos=True, freq_shift=0.0, round_t_
     emb = torch.cat([torch.sin(emb), torch.cos(emb)], dim=-1)
     if flip_sin_to_cos:
         emb = torch.cat([emb[:, half:], emb[:, :half]], dim=-1)
-    return emb.to(BF16)
+    return F.pad(emb, (0, dim - 2 * half)).to(BF16)  # odd dim: a trailing zero column
 
 
 def silu(x):
