@@ -21,8 +21,17 @@ def _alphas_cumprod(beta_start=0.00085, beta_end=0.012, n=1000, schedule="scaled
     return np.cumprod(1.0 - betas, axis=0)
 
 
+def _check_steps(num_inference_steps: int, num_train_timesteps: int):
+    """The "leading" spacing takes every (train // inference)-th training step: past num_train_timesteps the ratio is 0
+    and every step would land on the same timestep."""
+    if not 1 <= num_inference_steps <= num_train_timesteps:
+        raise ValueError(f"num_inference_steps must be in 1..{num_train_timesteps} (num_train_timesteps), got "
+                         f"{num_inference_steps}")
+
+
 class EulerDiscreteSchedule:
     def __init__(self, num_inference_steps: int, num_train_timesteps: int = 1000, steps_offset: int = 1):
+        _check_steps(num_inference_steps, num_train_timesteps)
         ac = _alphas_cumprod(n=num_train_timesteps)
         step_ratio = num_train_timesteps // num_inference_steps
         ts = (np.arange(0, num_inference_steps) * step_ratio).round()[::-1].copy().astype(np.float32) + steps_offset
@@ -81,9 +90,14 @@ class DDIMSchedule:
         if rescale_betas_zero_snr:
             betas = _rescale_zero_terminal_snr(betas)
         self.ac = np.cumprod(1.0 - betas, axis=0).astype(np.float32)
+        _check_steps(num_inference_steps, num_train_timesteps)
         step_ratio = num_train_timesteps // num_inference_steps
         self.timesteps = ((np.arange(0, num_inference_steps) * step_ratio).round()[::-1].copy().astype(np.int64)
                           + steps_offset)
+        if self.timesteps[0] >= num_train_timesteps:
+            # e.g. 1000 steps of 1000: the first timestep, 999 + steps_offset, has no alpha_prod_t
+            raise ValueError(f"{num_inference_steps} DDIM steps with steps_offset {steps_offset} reach timestep "
+                             f"{int(self.timesteps[0])}, past the last of {num_train_timesteps} training timesteps")
         self.step_ratio = step_ratio
         self.final_alpha = 1.0 if set_alpha_to_one else float(self.ac[0])
         self.init_noise_sigma = 1.0
@@ -105,6 +119,7 @@ class EulerKarrasVSchedule:
     "leading" spacing (init_noise_sigma = sqrt(sigma_max^2 + 1)).  Used by pipeline_svd (svd pipeline :600-602, :775)."""
 
     def __init__(self, num_inference_steps: int, sigma_min: float = 0.002, sigma_max: float = 700.0, rho: float = 7.0):
+        _check_steps(num_inference_steps, 1000)  # the control timesteps step by 1000 // num_inference_steps
         ramp = np.linspace(0, 1, num_inference_steps)
         lo, hi = sigma_min ** (1 / rho), sigma_max ** (1 / rho)
         sig = ((hi + ramp * (lo - hi)) ** rho).astype(np.float32)

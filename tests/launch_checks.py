@@ -15,12 +15,19 @@ argument; every scalar argument.  The first call with a key:
      bit-identical to the in-step output (a read of a guard band or stride gap picks up NaN there); group_norm, whose
      statistics are summed with float atomics, must pass its reference again instead; and every byte outside the
      argument views must keep its fill.
-Later calls with the same key are only counted.  A call without a verifier, or one its verifier cannot handle, fails.
+Later calls with the same key are only counted, except for the ops named in `every_call` (opt-in; the scheduler
+updates, whose per-step row changes while their key does not): those get their verdict on every call, and `on_call` (if
+given) sees the arguments of each such call before it runs.  `context` (default None) is a label the caller may set
+between calls, e.g. the conditioning-scale body a step runs: a launch is then first-call checked once per context, so a
+configuration two bodies share is verified on the data of each.  A call without a verifier, or one its verifier cannot
+handle, fails.
 Where the float64 reference of a whole launch would be too large, it is evaluated on the first, middle and last image /
 batch entry / sample (never on part of an image) and the row says so.
 
 tests/test_launch_census_gpu.py runs one step of each benchmark workload and the VAE at the pipelines' geometry under
-it; tests/test_launch_checks_cpu.py runs it over the emulated op layer and shows that it flags wrong variants.
+it; tests/test_schedule_census_gpu.py runs the benchmark batch sizes and whole schedules across both conditioning-scale
+bodies and with sparse key frames, the scheduler updates in `every_call`; tests/test_launch_checks_cpu.py runs it over
+the emulated op layer and shows that it flags wrong variants.
 """
 from __future__ import annotations
 
@@ -40,6 +47,7 @@ OPS = ("linear", "conv2d", "temporal_conv", "attention", "temporal_attention", "
        "i2vgen_latent_encoder", "vae_latents")
 OUT_ARGS = ("out", "latents_out", "model_in_next")
 SAMPLE_BYTES = 3 << 29  # float64 reference of a launch above this: evaluated on the first, middle and last entry
+LINEAR_SAMPLE_BYTES = 6 << 30  # linear: a float64 [M, max(K, N)] above this (the video UNets at benchmark batch)
 
 
 def _ops():
@@ -66,7 +74,14 @@ def _sample(n, bytes_per_item):
 # with some arguments changed) -> (records, sampled)
 # ----------------------------------------------------------------------------------------------------------------------
 def _v_linear(a, out, rerun):
-    return kc.linear_verdict("linear", a, out, rerun), False
+    m, k = a["x"].shape
+    rows = None
+    if 8 * m * max(k, a["w"].shape[0]) > LINEAR_SAMPLE_BYTES:  # w rows: GEGLU's pre-activation is twice the output
+        # rows of the first, middle and last image: the rows of one row-vector entry, or of one 64x64 / 72x128 latent
+        per = a["rows_per_vec"] if a["rowvec"] is not None else math.gcd(m, 4096)
+        n = m // per
+        rows = torch.cat([torch.arange(i * per, (i + 1) * per, device=out.device) for i in sorted({0, n // 2, n - 1})])
+    return kc.linear_verdict("linear", a, out, rerun, rows=rows), rows is not None
 
 
 def _v_conv2d(a, out, rerun):
@@ -410,8 +425,8 @@ def _same_bits(a, b):
 
 
 class Row:
-    def __init__(self, op, key):
-        self.op, self.key, self.launches = op, key, 0
+    def __init__(self, op, key, context=None):
+        self.op, self.key, self.context, self.launches, self.verdicts = op, key, context, 0, 0
         self.worst, self.where, self.sampled, self.ok, self.why = 0.0, "", False, True, []
         self.notes = {}
 
@@ -435,8 +450,11 @@ class Row:
 class Recorder:
     """with Recorder() as rec: ... -- every launch through ctrl_adapter_b200.ops is keyed, the first of each key checked"""
 
-    def __init__(self, sync=None):
-        self.rows = {}
+    def __init__(self, sync=None, every_call=(), on_call=None):
+        self.rows = {}  # config key (or (context, config key) while a context is set) -> Row
+        self.context = None
+        self.every_call = frozenset(every_call)
+        self.on_call = on_call
         self._busy = False
         self._saved = {}
         self._sync = sync or kc._sync
@@ -466,18 +484,38 @@ class Recorder:
             bound.apply_defaults()
             a = dict(bound.arguments)
             key = config_key(name, a)
-            row = self.rows.get(key)
+            every = name in self.every_call
+            if every and self.on_call is not None:
+                self.on_call(name, a)
+            rk = key if self.context is None else (self.context, key)
+            row = self.rows.get(rk)
             if row is not None:
                 row.launches += 1
-                return fn(*args, **kw)
-            row = self.rows[key] = Row(name, key)
-            row.launches = 1
+                if not every:
+                    return fn(*args, **kw)
+            else:
+                row = self.rows[rk] = Row(name, key, self.context)
+                row.launches = 1
             self._busy = True
             try:
-                return self._first(name, fn, a, row)
+                return (self._again if row.launches > 1 else self._first)(name, fn, a, row)
             finally:
                 self._busy = False
         return wrapped
+
+    def _again(self, name, fn, a, row):
+        """a later call of an `every_call` op: its verdict against the reference on the pre-call inputs"""
+        clone = _Clone(a)
+        pre = {**clone.args(a), **{k: a[k] for k in OUT_ARGS if k in a}}
+        ret = fn(**a)
+        self._sync()
+        try:
+            recs, _ = VERIFIERS[name](pre, ret, None)
+            row.add(recs)
+            row.verdicts += 1
+        except Exception as e:
+            row.fail(f"{type(e).__name__}: {e}"[:300])
+        return ret
 
     def _first(self, name, fn, a, row):
         clone = _Clone(a)
@@ -492,6 +530,7 @@ class Recorder:
                 raise NotImplementedError(f"no verifier for ops.{name}")
             recs, row.sampled = verify(pre, ret, lambda **changes: fn(**{**clone.args(a), **changes}))
             row.add(recs)
+            row.verdicts += 1
             for k in OUT_ARGS:
                 t = a.get(k)
                 if torch.is_tensor(t) and not clone.untouched_around(t, outs):
@@ -523,7 +562,8 @@ class Recorder:
         lines = [f"{'op':<22} {'launches':>8} {'err/tol':>8}  {'sampled':<7} {'where':<28} configuration"]
         for row in sorted(self.rows.values(), key=lambda r: (r.op, -r.worst)):
             lines.append(f"{row.op:<22} {row.launches:>8} {row.worst:>8.3f}  {'yes' if row.sampled else '':<7} "
-                         f"{row.where[:28]:<28} {key_summary(row.key)}" +
+                         f"{row.where[:28]:<28} " + ("" if row.context is None else f"[{row.context}] ") +
+                         key_summary(row.key) + ("" if row.verdicts <= 1 else f" verdicts={row.verdicts}") +
                          "".join(f" {k}={v:.3g}" for k, v in row.notes.items()) + ("" if row.ok else f"  FAIL {row.why}"))
         return "\n".join(lines)
 

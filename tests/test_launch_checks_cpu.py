@@ -255,3 +255,104 @@ def test_census_catches_wrong_variant(variant):
     print(f"\n{variant}: caught by " + ("; ".join(f"{r.op} {lc.key_summary(r.key)} [{r.where}]" for r in bad[:3])
                                        or "NOTHING"))
     assert bad, f"no launch notices: {variant}"
+
+
+# ---- the CFG + scheduler updates over whole schedules: a verdict on every call (Recorder every_call) ----
+CFG_OPS = ("cfg_euler", "cfg_euler_v", "cfg_ddim")
+
+
+def _schedule_updates(kind, steps, wrong=None, every_call=()):
+    """the last launch of a loop's step over the steps `steps` of its schedule, made as the loop makes it: one step row
+    refreshed from the table before each call, the latents updated in place, the next model input written"""
+    from ctrl_adapter_b200 import schedulers as S
+    sch = {"euler": lambda: S.EulerDiscreteSchedule(50), "euler_v": lambda: S.EulerKarrasVSchedule(25),
+           "ddim": lambda: S.DDIMSchedule(50)}[kind]()
+    shape = (2, 3, 4, 6, 8)
+    eu, et = _r(*shape, seed=30), _r(*shape, seed=31)
+    table = torch.from_numpy(sch.table())
+    row = table[0].clone()
+    lat = (torch.randn(*shape, generator=torch.Generator().manual_seed(32)) * sch.init_noise_sigma).to(BF16).float()
+    nxt = torch.empty(shape, dtype=BF16)
+    with emu.patched_ops() as ops:
+        for name, fn in (wrong or {}).items():
+            setattr(ops, name, fn)
+        with lc.Recorder(every_call=every_call) as rec:
+            for i in steps:
+                row.copy_(table[i])
+                if kind == "euler":
+                    ops.cfg_euler(eu, et, lat, 5.0, row, latents_out=lat, model_in_next=nxt)
+                elif kind == "euler_v":
+                    ops.cfg_euler_v(eu, et, lat, torch.linspace(1.0, 3.0, 3).to(BF16).float(), 3, row, latents_out=lat,
+                                    model_in_next=nxt)
+                else:
+                    ops.cfg_ddim(eu, et, lat, 9.0, row, latents_out=lat, model_in_next=nxt, v_prediction=True)
+    return rec, len(table)
+
+
+@pytest.mark.parametrize("kind", ["euler", "euler_v", "ddim"])
+def test_every_call_verdict_covers_every_row(kind):
+    """with every_call, each call of a whole schedule gets its verdict (one key, as many verdicts as steps); without it
+    only the first does, as before"""
+    rec, n = _schedule_updates(kind, range({"euler_v": 25}.get(kind, 50)), every_call=CFG_OPS)
+    assert not rec.failures(), rec.table()
+    assert len(rec.rows) == 1 and [r.verdicts for r in rec.rows.values()] == [n]
+    rec, n = _schedule_updates(kind, range(n))
+    assert not rec.failures() and [(r.launches, r.verdicts) for r in rec.rows.values()] == [(n, 1)]
+
+
+def _euler_sigma_next_zero_no_step(eps_uncond, eps_text, latents, guidance, step_row, latents_out=None,
+                                   model_in_next=None, round_latents_bf16=True):
+    """sigma_next == 0 (the last step) treated as "no step": the latents are left as they are"""
+    if float(step_row[2]) != 0.0:
+        return emu.cfg_euler(eps_uncond, eps_text, latents, guidance, step_row, latents_out, model_in_next,
+                             round_latents_bf16)
+    y = latents.clone()
+    if model_in_next is not None:
+        model_in_next.copy_((y / float(step_row[3].to(BF16))).to(BF16))
+    return _into(y, latents_out)
+
+
+def _ddim_final_alpha_as_alpha_t(eps_uncond, eps_text, latents, guidance, step_row, latents_out=None,
+                                 model_in_next=None, round_latents_bf16=True, v_prediction=False):
+    """alpha_prod_prev == 1 (set_alpha_to_one on the last step) replaced by alpha_prod_t"""
+    if float(step_row[2]) == 1.0:
+        step_row = step_row.clone()
+        step_row[2] = step_row[1]
+    return emu.cfg_ddim(eps_uncond, eps_text, latents, guidance, step_row, latents_out, model_in_next,
+                        round_latents_bf16, v_prediction)
+
+
+SCHEDULE_VARIANTS = {
+    "cfg_euler: sigma_next == 0 taken as no step": ("euler", {"cfg_euler": _euler_sigma_next_zero_no_step}),
+    "cfg_ddim: alpha_prev == 1 replaced by alpha_t": ("ddim", {"cfg_ddim": _ddim_final_alpha_as_alpha_t}),
+}
+
+
+@pytest.mark.parametrize("variant", list(SCHEDULE_VARIANTS))
+def test_every_call_verdict_catches_end_of_schedule_variant(variant):
+    """special-cased end-of-schedule arithmetic: invisible to the step-0 census (first call of the key only), caught
+    when every step's update gets its verdict"""
+    kind, wrong = SCHEDULE_VARIANTS[variant]
+    old, n = _schedule_updates(kind, [0], wrong)
+    assert not old.failures(), f"the step-0 census should not see it: {variant}"
+    rec, _ = _schedule_updates(kind, range(n), wrong, every_call=CFG_OPS)
+    bad = rec.failures()
+    print(f"\n{variant}: step-0 census passes; every-call census caught by "
+          + ("; ".join(f"{r.op} {lc.key_summary(r.key)} [{r.where}] after {r.verdicts} verdicts" for r in bad[:3])
+             or "NOTHING"))
+    assert bad, f"no verdict notices: {variant}"
+
+
+@pytest.mark.parametrize("wrong", [None, "linear: row vector at the 128-row tile origin"])
+def test_linear_rows_sampled(wrong, monkeypatch):
+    """linear launches too large for a whole float64 reference (the video UNets at benchmark batch) are verified on the
+    rows of their first, middle and last image: the emulated census passes that way, and a wrong row vector is still
+    caught"""
+    monkeypatch.setattr(lc, "LINEAR_SAMPLE_BYTES", 0)
+    rec = _run(VARIANTS[wrong] if wrong else None)
+    linear = [r for r in rec.rows.values() if r.op == "linear"]
+    assert linear and all(r.sampled for r in linear)
+    bad = rec.failures()
+    print(f"\nlinear rows sampled, {wrong or 'correct emulation'}: "
+          + ("; ".join(f"{r.op} {lc.key_summary(r.key)}: {r.why}" for r in bad[:2]) or "passes"))
+    assert bool(bad) == bool(wrong)
