@@ -46,7 +46,7 @@ int launched(cudaError_t e, const char* what) {
 }
 
 int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-              const cuuint32_t* box) {
+              const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return fail(CA_ERR_INVALID, "tensor base not 16-byte aligned");
   for (int i = 0; i + 1 < rank; ++i)
     if (strides_bytes[i] % 16 != 0) return fail(CA_ERR_INVALID, "tensor stride %d (%llu B) not a multiple of 16", i + 1,
@@ -55,7 +55,7 @@ int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims
   if (!fn) return fail(CA_ERR_CUDA, "cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     return fail(CA_ERR_CUDA,

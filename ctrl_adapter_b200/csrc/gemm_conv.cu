@@ -118,14 +118,42 @@ extern "C" int ca_gemm(const ca_gemm_desc* d, void* cuda_stream) {
     int rc = make_tmap(&tw, d->w, 2, dims, strides, box);
     if (rc) return rc;
   }
+  // Residual and blend source of the bf16 (non-GEGLU) epilogue on the aligned path: 5-D maps over the output's row
+  // space that load 32 columns x the tile's row box, unswizzled, so the storers read them from shared memory.  A row
+  // dim that has more than one point but stride 0 (a broadcast) cannot be expressed: such calls keep the
+  // per-chunk global loads.
+  CUtensorMap tr, tb;
+  memset(&tr, 0, sizeof(tr));
+  memset(&tb, 0, sizeof(tb));
+  if (p.vec_ok && !p.out_fp32 && !geglu && (p.residual || p.blend_src)) {
+    cuuint64_t dims[5] = {static_cast<cuuint64_t>(p.n_out), (cuuint64_t)p.odim[0], (cuuint64_t)p.odim[1],
+                          (cuuint64_t)p.odim[2], (cuuint64_t)p.odim[3]};
+    cuuint64_t strides[4];
+    bool ok = true;
+    for (int i = 0; i < 4; ++i) {
+      strides[i] = static_cast<cuuint64_t>(p.rstride[i]) * 2;
+      if (p.rstride[i] < 0 || (p.rstride[i] == 0 && p.odim[i] > 1)) ok = false;
+      if (p.odim[i] == 1) strides[i] = i ? strides[i - 1] : (static_cast<cuuint64_t>(p.n_out) * 2 + 15) / 16 * 16;
+    }
+    cuuint32_t box[5] = {32, (cuuint32_t)d->box[0], (cuuint32_t)d->box[1], (cuuint32_t)d->box[2], (cuuint32_t)d->box[3]};
+    if (ok && p.residual) {
+      int rc = make_tmap(&tr, p.residual, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+      if (rc) return rc;
+    }
+    if (ok && p.blend_src) {
+      int rc = make_tmap(&tb, p.blend_src, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+      if (rc) return rc;
+    }
+    p.ops_tma = ok ? 1 : 0;
+  }
   const long long sms = num_sms();
   const int grid = static_cast<int>(tiles < sms ? tiles : sms);
   cudaError_t e;
   switch (bn) {
-    case 64: e = launch_gemm_bn64(ta[0], ta[1], tw, p, grid, stream); break;
-    case 128: e = launch_gemm_bn128(ta[0], ta[1], tw, p, grid, stream); break;
-    case 160: e = launch_gemm_bn160(ta[0], ta[1], tw, p, grid, stream); break;
-    default: e = launch_gemm_bn256(ta[0], ta[1], tw, p, grid, stream); break;
+    case 64: e = launch_gemm_bn64(ta[0], ta[1], tw, tr, tb, p, grid, stream); break;
+    case 128: e = launch_gemm_bn128(ta[0], ta[1], tw, tr, tb, p, grid, stream); break;
+    case 160: e = launch_gemm_bn160(ta[0], ta[1], tw, tr, tb, p, grid, stream); break;
+    default: e = launch_gemm_bn256(ta[0], ta[1], tw, tr, tb, p, grid, stream); break;
   }
   return launched(e, "gemm_conv launch");
 }

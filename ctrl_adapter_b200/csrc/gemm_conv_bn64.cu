@@ -2,8 +2,8 @@
 #include "gemm_conv_kernel.cuh"
 
 namespace ca {
-cudaError_t launch_gemm_bn64(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream) {
-  return launch_bn<64>(a0, a1, w, p, grid, stream);
+cudaError_t launch_gemm_bn64(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                             const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream) {
+  return launch_bn<64>(a0, a1, w, res, blend, p, grid, stream);
 }
 }  // namespace ca

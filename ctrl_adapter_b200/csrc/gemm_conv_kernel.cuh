@@ -13,8 +13,12 @@
 //                             it runs ahead into the next tile's ring slots while the current tile is written out
 //   warpgroup 0, warps 1-3  : storers (bf16 outputs).  Per tile: wait on `staged`, then read the staged tile, add
 //                             row vector / residual / AlphaBlender with their bf16 roundings and write the output with
-//                             16-byte loads and stores (element-wise when ca_gemm finds a pointer or stride that is
-//                             not 16-byte aligned), skipping rows outside the output box; then arrive on `drained`
+//                             16-byte stores (element-wise when ca_gemm finds a pointer or stride that is not 16-byte
+//                             aligned), skipping rows outside the output box; then arrive on `drained`.  On the
+//                             aligned path residual and blend source come by TMA into a ring of 32-column operand
+//                             slabs (kOps instantiation, gemm_drain_tile_ops), and storer 0 issues the first slabs of
+//                             a tile before the storers wait on `staged`, so their latency hides behind the main loop;
+//                             without kOps every 16-byte chunk waits on its own global loads (gemm_drain_tile)
 //   warpgroups 1, 2         : consumers.  Warpgroup g issues m64nBNk16 wgmma for rows [64g, 64g + 64) of the tile with
 //                             both operands read from the 128B-swizzled ring, accumulates in registers, and releases
 //                             a ring slot as soon as the wgmma that read it have retired.  After the last k-iteration
@@ -41,7 +45,7 @@ static constexpr int kStorerThreads = 96;     // warps 1-3 of warpgroup 0
 
 enum GemmEpilogue { kEpiBf16 = 0, kEpiGeglu = 1, kEpiF32 = 2 };
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool kOps = false>
 struct GemmCfg {
   static constexpr uint32_t kABytes = kBM * kBK * 2;  // 16 KB
   static constexpr uint32_t kBBytes = BN * kBK * 2;   // a multiple of the 1 KB swizzle atom for every BN used
@@ -56,13 +60,21 @@ struct GemmCfg {
   static constexpr uint32_t kPitch = kOutCols * 2 + (kSwizzle ? 0 : 16);
   static constexpr uint32_t kStagingBytes = kStaged ? kBM * kPitch : 0;
   static constexpr uint32_t kBiasBytes = kStaged ? BN * 4 : 0;
-  // 227 KB per block on H100, minus alignment slack, barriers, staging tile and bias: BN 256 keeps 3 ring stages
-  // (4 for GEGLU, whose staging tile is half as wide)
-  static constexpr uint32_t kBudget = 232448 - 1024 - 256 - kStagingBytes - kBiasBytes;
+  // kOps (bf16 epilogue with a residual and / or blend source, aligned path): a ring of kOpSlabs 8 KB slabs, each
+  // [kBM rows][32 columns] of one source, which TMA fills ahead of the storers.  BN 256 and 64 take 2 slabs, which
+  // fit beside their ring stages; BN 160 and 128 give up one ring stage either way and then have room for 4.
+  static constexpr int kOpSlabs = !kOps ? 0 : (BN == 160 || BN == 128) ? 4 : 2;
+  static constexpr uint32_t kOpSlabBytes = kBM * 32 * 2;
+  static constexpr uint32_t kOpBytes = kOpSlabs * kOpSlabBytes;
+  // 227 KB per block on H100, minus alignment slack, barriers, staging tile, bias and operand slabs: BN 256 keeps 3
+  // ring stages (4 for GEGLU, whose staging tile is half as wide)
+  static constexpr uint32_t kBudget = 232448 - 1024 - 256 - kStagingBytes - kBiasBytes - kOpBytes;
   static constexpr int kStagesRaw = kBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
   static constexpr uint32_t kSmemBytes =
-      kStages * kStageBytes + kStagingBytes + kBiasBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+      kStages * kStageBytes + kStagingBytes + kBiasBytes + kOpBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(EPI == kEpiBf16 || !kOps, "operand slabs are for the plain bf16 epilogue");
+  static_assert(2 * kStages + 2 + 4 <= 32, "barriers fit in 256 bytes");
   // registers per thread after setmaxnreg: 128 * kWg0Regs + 256 * kConsumerRegs = 384 * 168
   static constexpr int kWg0Regs = kStaged ? 72 : 40;
   static constexpr int kConsumerRegs = kStaged ? 216 : 232;
@@ -190,6 +202,63 @@ __device__ __forceinline__ void gemm_drain_tile(const GemmParams& p, const uint8
   }
 }
 
+// Storers, aligned path with residual / blend source in shared memory: the tile's valid columns go in 32-column
+// groups.  Group g's slabs (one per source) sit in slab slots [nops (g % G), nops (g % G) + nops), G = kOpSlabs / nops
+// groups ahead, filled by TMA on op_bar[g % G].  Storer 0 issues a group's loads as soon as its slots are free: the
+// first G groups of a tile before the storers wait on `staged`, so that they arrive while the consumers are still in
+// the main loop.  The arithmetic is gemm_drain_tile's.
+template <class Cfg>
+__device__ __forceinline__ void gemm_drain_tile_ops(const GemmParams& p, const CUtensorMap* tmap_r,
+                                                    const CUtensorMap* tmap_b, const uint8_t* staging, uint8_t* op_smem,
+                                                    uint64_t* op_bar, uint32_t& op_phase, uint64_t* staged_bar,
+                                                    uint32_t staged_phase, int tn, const int (&org)[4],
+                                                    const int (&lb)[4], int s, float alpha_s, float alpha_t) {
+  const bool rv_on = p.rowvec != nullptr, res_on = p.residual != nullptr, blend_on = p.blend_src != nullptr;
+  const int nops = (res_on ? 1 : 0) + (blend_on ? 1 : 0);
+  const int ahead = Cfg::kOpSlabs / nops;
+  __nv_bfloat16* out = static_cast<__nv_bfloat16*>(p.out);
+  const int col0 = tn * Cfg::kOutCols;
+  const int cols = min(Cfg::kOutCols, p.n_out - col0);
+  const int groups = (cols + 31) >> 5;
+  auto issue = [&](int g) {
+    const int k = g % ahead;
+    uint8_t* dst = op_smem + k * nops * Cfg::kOpSlabBytes;
+    mbar_arrive_expect_tx(&op_bar[k], nops * Cfg::kOpSlabBytes);
+    if (res_on) tma_load_5d(dst, tmap_r, &op_bar[k], col0 + 32 * g, org[0], org[1], org[2], org[3]);
+    if (blend_on)
+      tma_load_5d(dst + (res_on ? Cfg::kOpSlabBytes : 0), tmap_b, &op_bar[k], col0 + 32 * g, org[0], org[1], org[2],
+                  org[3]);
+  };
+  if (s == 0)
+    for (int g = 0; g < min(ahead, groups); ++g) issue(g);
+  mbar_wait(staged_bar, staged_phase);
+  for (int g = 0; g < groups; ++g) {
+    const int k = g % ahead;
+    mbar_wait(&op_bar[k], (op_phase >> k) & 1);
+    op_phase ^= 1u << k;
+    const uint8_t* slab = op_smem + k * nops * Cfg::kOpSlabBytes;
+    // 128 rows x 4 chunks: a quarter warp reads two whole 64-byte slab rows
+    for (int q = s; q < kBM * 4; q += kStorerThreads) {
+      const int r = q >> 2, c = 4 * g + (q & 3), col = col0 + 8 * c;
+      const GemmRow gr = gemm_row(p, org, lb, r);
+      if (!gr.ok || col >= p.n_out) continue;
+      uint4 rv, rs, bs;
+      if (rv_on) rv = ld8_bf16<true>(p.rowvec + gr.rv + col);
+      const uint8_t* o = slab + r * 64 + (q & 3) * 16;
+      if (res_on) rs = *reinterpret_cast<const uint4*>(o);
+      if (blend_on) bs = *reinterpret_cast<const uint4*>(o + (res_on ? Cfg::kOpSlabBytes : 0));
+      uint4 v = *reinterpret_cast<const uint4*>(staging + Cfg::chunk_off(r, c));
+      v.x = gemm_finish_word(v.x, rv_on, rv.x, res_on, rs.x, blend_on, bs.x, alpha_s, alpha_t);
+      v.y = gemm_finish_word(v.y, rv_on, rv.y, res_on, rs.y, blend_on, bs.y, alpha_s, alpha_t);
+      v.z = gemm_finish_word(v.z, rv_on, rv.z, res_on, rs.z, blend_on, bs.z, alpha_s, alpha_t);
+      v.w = gemm_finish_word(v.w, rv_on, rv.w, res_on, rs.w, blend_on, bs.w, alpha_s, alpha_t);
+      st8_bf16<true>(out + gr.out + col, v);
+    }
+    named_bar_sync(2, kStorerThreads);  // every storer is done with the group's slots
+    if (s == 0 && g + ahead < groups) issue(g + ahead);
+  }
+}
+
 // fp32 output, straight from the accumulators.  Thread holds rows (r0, r0 + 8) x columns 8 j + 2 (lane & 3) + {0, 1}.
 // Rounded to bf16 only where the reference's chain is bf16: after SiLU and after the row vector.
 template <int BN>
@@ -287,11 +356,12 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
   }
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool kOps>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1,
-                 const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
-  using Cfg = GemmCfg<BN, EPI>;
+                 const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_r,
+                 const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+  using Cfg = GemmCfg<BN, EPI, kOps>;
   CA_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -301,11 +371,13 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;         // kStages x BN*128 B
   uint8_t* staging = smem + Cfg::kStages * Cfg::kStageBytes;    // kBM x kPitch B (bf16 outputs)
   float* bias_s = reinterpret_cast<float*>(staging + Cfg::kStagingBytes);  // [BN] (bf16 outputs)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes + Cfg::kBiasBytes);
+  uint8_t* op_smem = staging + Cfg::kStagingBytes + Cfg::kBiasBytes;      // kOpSlabs x 8 KB (kOps)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(op_smem + Cfg::kOpBytes);
   uint64_t* full_bar = bars;                        // [kStages]
   uint64_t* empty_bar = bars + Cfg::kStages;        // [kStages]
   uint64_t* staged_bar = bars + 2 * Cfg::kStages;   // consumers -> storers: the staging tile holds tile i
   uint64_t* drained_bar = staged_bar + 1;           // storers -> consumers: the staging tile may be overwritten
+  uint64_t* op_bar = staged_bar + 2;                // [4] TMA -> storers: a group's operand slabs have landed (kOps)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -326,6 +398,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
     }
     mbar_init(staged_bar, kConsumerThreads);
     mbar_init(drained_bar, kStorerThreads);
+    if (kOps)
+      for (int k = 0; k < 4; ++k) mbar_init(&op_bar[k], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -380,10 +454,21 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
       }
       const int lb[4] = {__ffs(p.box[0]) - 1, __ffs(p.box[1]) - 1, __ffs(p.box[2]) - 1, __ffs(p.box[3]) - 1};
       const int kind = (p.rowvec != nullptr ? 1 : 0) | (p.residual != nullptr ? 2 : 0) | (p.blend_src != nullptr ? 4 : 0);
-      uint32_t phase = 0;
+      if (kOps && s == 0) {
+        if (p.residual) tma_prefetch_desc(&tmap_r);
+        if (p.blend_src) tma_prefetch_desc(&tmap_b);
+      }
+      uint32_t phase = 0, op_phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int tn, org[4];
         tile_coords(tile, tn, org);
+        if constexpr (kOps) {
+          gemm_drain_tile_ops<Cfg>(p, &tmap_r, &tmap_b, staging, op_smem, op_bar, op_phase, staged_bar, phase, tn,
+                                   org, lb, s, alpha_s, alpha_t);
+          mbar_arrive(drained_bar);
+          phase ^= 1;
+          continue;
+        }
         mbar_wait(staged_bar, phase);
         if (!p.vec_ok) {
           gemm_drain_tile<Cfg, false, false, false, false>(p, staging, tn, org, lb, s, alpha_s, alpha_t);
@@ -461,28 +546,30 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
   }
 }
 
-template <int BN, int EPI>
-static cudaError_t launch_epi(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, EPI>;
+template <int BN, int EPI, bool kOps = false>
+static cudaError_t launch_epi(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w,
+                              const CUtensorMap& res, const CUtensorMap& blend, const GemmParams& p, int grid,
+                              cudaStream_t stream) {
+  using Cfg = GemmCfg<BN, EPI, kOps>;
   static bool attr_set = false;
-  auto kern = gemm_conv_kernel<BN, EPI>;
+  auto kern = gemm_conv_kernel<BN, EPI, kOps>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(Cfg::kSmemBytes));
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  return launch_pdl(kern, grid, kGemmThreads, Cfg::kSmemBytes, stream, a0, a1, w, p);
+  return launch_pdl(kern, grid, kGemmThreads, Cfg::kSmemBytes, stream, a0, a1, w, res, blend, p);
 }
 
 // one translation unit per BN (gemm_conv_bn*.cu) instantiates its kernels through this
 template <int BN>
-static cudaError_t launch_bn(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                             int grid, cudaStream_t stream) {
-  if (p.out_fp32) return launch_epi<BN, kEpiF32>(a0, a1, w, p, grid, stream);
-  if (p.act == CA_ACT_GEGLU) return launch_epi<BN, kEpiGeglu>(a0, a1, w, p, grid, stream);
-  return launch_epi<BN, kEpiBf16>(a0, a1, w, p, grid, stream);
+static cudaError_t launch_bn(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                             const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream) {
+  if (p.out_fp32) return launch_epi<BN, kEpiF32>(a0, a1, w, res, blend, p, grid, stream);
+  if (p.act == CA_ACT_GEGLU) return launch_epi<BN, kEpiGeglu>(a0, a1, w, res, blend, p, grid, stream);
+  if (p.ops_tma) return launch_epi<BN, kEpiBf16, true>(a0, a1, w, res, blend, p, grid, stream);
+  return launch_epi<BN, kEpiBf16>(a0, a1, w, res, blend, p, grid, stream);
 }
 
 }  // namespace ca

@@ -16,9 +16,10 @@ namespace ca {
 int fail(int code, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
 // CA_OK for cudaSuccess, else CA_ERR_CUDA with "what: <CUDA error>"
 int launched(cudaError_t e, const char* what);
-// bf16 tensor map, 128B swizzle, zero OOB fill. dims/strides fastest-first; strides in BYTES for dims 1..rank-1.
+// bf16 tensor map, 128B swizzle unless `swizzle` says otherwise, zero OOB fill. dims/strides fastest-first; strides
+// in BYTES for dims 1..rank-1.
 int make_tmap(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-              const cuuint32_t* box);
+              const cuuint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 int num_sms();
 // argument checks: a pointer the kernel accesses in `bytes`-wide vectors (a null pointer passes), and the largest
 // gridDim.y / gridDim.z a launch may have
@@ -45,6 +46,7 @@ struct GemmParams {
   int act;
   int out_fp32;
   int vec_ok;             // bf16 output: out / residual / blend_src / rowvec bases and strides allow 16-byte access
+  int ops_tma;            // bf16, non-GEGLU, vec_ok: residual / blend_src come through their tensor maps
   float out_scale;
   const float* bias;               // [weight rows] fp32
   const __nv_bfloat16* rowvec;     // broadcast add, indexed through vstride
@@ -55,13 +57,13 @@ struct GemmParams {
 };
 
 // one per N tile width, each in its own translation unit so that the kernel instantiations compile in parallel
-cudaError_t launch_gemm_bn64(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                             int grid, cudaStream_t stream);
-cudaError_t launch_gemm_bn128(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream);
-cudaError_t launch_gemm_bn160(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream);
-cudaError_t launch_gemm_bn256(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const GemmParams& p,
-                              int grid, cudaStream_t stream);
+cudaError_t launch_gemm_bn64(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                             const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream);
+cudaError_t launch_gemm_bn128(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                              const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream);
+cudaError_t launch_gemm_bn160(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                              const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream);
+cudaError_t launch_gemm_bn256(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& w, const CUtensorMap& res,
+                              const CUtensorMap& blend, const GemmParams& p, int grid, cudaStream_t stream);
 
 }  // namespace ca

@@ -172,6 +172,15 @@ def _fill_epilogue(d: GemmDesc, *, bias, act, out_scale, rowvec, rowvec_strides,
         d.res_strides[i] = res_strides[i] if res_strides else 0
 
 
+def _epilogue_note(w_rows, act, bn, residual, rowvec, blend_src):
+    """Profiler shape note of a GEMM's N tile and epilogue operands.  bn 0 is resolved by ca_gemm's rule."""
+    if bn == 0:
+        bn = next((b for b in (256, 160, 128) if w_rows % b == 0), 64 if w_rows <= 64 else 128 if w_rows <= 128 else 256)
+        bn = 256 if act == ACT_GEGLU else bn
+    return (f"bn{bn} res{int(residual is not None)} rv{int(rowvec is not None)} "
+            f"blend{int(blend_src is not None)}")
+
+
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, *, act: int = ACT_NONE,
            residual: Optional[torch.Tensor] = None, rowvec: Optional[torch.Tensor] = None, rows_per_vec: int = 0,
            blend_src: Optional[torch.Tensor] = None, blend_alpha: Optional[torch.Tensor] = None,
@@ -227,7 +236,7 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     _fill_epilogue(d, bias=bias, act=act, out_scale=out_scale, rowvec=rowvec, rowvec_strides=rvs, residual=residual,
                    blend_src=blend_src, res_strides=rs, blend_alpha=blend_alpha)
     if PROFILER.active:
-        NOTE[0] = f"linear m{m} k{k} n{wr} act{act} res{int(residual is not None)}"
+        NOTE[0] = f"linear m{m} k{k} n{wr} act{act} {_epilogue_note(wr, act, bn, residual, rowvec, blend_src)}"
     _launch("gemm", 2.0 * m * k * wr, 2.0 * (m * k + wr * k + m * n_out), "ca_gemm", C.byref(d), _stream())
     return out
 
@@ -312,7 +321,8 @@ def conv2d(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor]
                    residual=residual, blend_src=blend_src,
                    res_strides=os_ if (residual is not None or blend_src is not None) else None, blend_alpha=blend_alpha)
     if PROFILER.active:
-        NOTE[0] = f"conv{ksize} s{stride} n{n} {h}x{w_} c{c}+{c2}->{cout} box{bw}x{bh}x{bnn}"
+        NOTE[0] = (f"conv{ksize} s{stride} n{n} {h}x{w_} c{c}+{c2}->{cout} box{bw}x{bh}x{bnn} "
+                   f"{_epilogue_note(cout, act, bn, residual, rowvec, blend_src)}")
     _launch("gemm", 2.0 * n * ho * wo * ntaps * (c + c2) * cout,
             2.0 * (n * h * w_ * (c + c2) + w_packed.numel() + n * ho * wo * cout), "ca_gemm", C.byref(d), _stream())
     return out

@@ -1,5 +1,6 @@
 """Launches single hot kernels at the BASELINE config-2 shapes (for ncu captures and quick CUDA-event timings).
-usage: python scripts/prof_kernels.py attn|attn1k|attn77|geglu|lin_small|lin_res|conv [--time]"""
+usage: python scripts/prof_kernels.py attn|attn1k|attn77|geglu|lin_small|lin_res|conv [--time] [--no-res]
+--no-res drops the residual of lin_small / lin_res: the same GEMM with a plain epilogue."""
 import math
 import os
 import sys
@@ -12,6 +13,7 @@ from ctrl_adapter_b200 import ops  # noqa: E402
 BF16 = torch.bfloat16
 which = sys.argv[1]
 do_time = "--time" in sys.argv
+no_res = "--no-res" in sys.argv
 torch.manual_seed(0)
 dev = "cuda"
 
@@ -35,12 +37,12 @@ elif which == "geglu":
     flops = 2.0 * 16384 * 1280 * 10240
 elif which == "lin_small":
     x, w, bias = rnd(65536, 640), rnd(640, 640, scale=1 / math.sqrt(640)), torch.zeros(640, device=dev)
-    res = rnd(65536, 640)
+    res = None if no_res else rnd(65536, 640)
     fn = lambda: ops.linear(x, w, bias, residual=res)  # noqa: E731
     flops = 2.0 * 65536 * 640 * 640
 elif which == "lin_res":
     x, w, bias = rnd(16384, 1280), rnd(1280, 1280, scale=1 / math.sqrt(1280)), torch.zeros(1280, device=dev)
-    res = rnd(16384, 1280)
+    res = None if no_res else rnd(16384, 1280)
     fn = lambda: ops.linear(x, w, bias, residual=res)  # noqa: E731
     flops = 2.0 * 16384 * 1280 * 1280
 elif which.startswith("conv"):  # conv or conv:<bn>
