@@ -108,7 +108,8 @@ typedef struct ca_attention_desc {
   const void* q; const void* k; const void* v; void* out;
   int32_t batch, heads, lq, lk;
   int32_t head_dim_pad;                 /* 64, 128 or 192 */
-  float scale;                          /* softmax scale (1/sqrt(true head dim)) */
+  float scale;                          /* softmax scale (1/sqrt(true head dim)): positive and finite, as is
+                                           scale * log2(e) (the softmax works in base 2); others -> CA_ERR_INVALID */
   int64_t q_row_stride, q_batch_stride; /* elements */
   int64_t k_row_stride, k_batch_stride;
   int64_t v_row_stride, v_batch_stride;
