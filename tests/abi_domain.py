@@ -11,11 +11,17 @@ restating the dispatch rules of csrc/ in Python (gemm_bn, layernorm_variant, ...
 argument, every branch, and a few seeded interior points.  Calls that `ops` cannot express (LayerNorm in place) go to
 the C entry point through `_lib` with the header's argument names.  small=True: reduced sizes for the CPU run over
 tests/ops_emulator.py, as in kernel_checks.layout_cases(small=True).
+
+On the GPU the predictions are checked against what ran: KernelTrace records the kernels of each case's first launch,
+kernel_labels parses their template arguments into the name-visible labels, visible_parts gives the labels a predicted
+branch implies, and observed_dispatch requires the two to agree case by case.
 """
 from __future__ import annotations
 
 import ctypes as C
 import random
+import re
+import time
 from dataclasses import dataclass, field
 from typing import Callable, Tuple
 
@@ -40,8 +46,21 @@ def gemm_bn(w_rows, geglu=False, bn=0):
     return 64 if w_rows <= 64 else 128 if w_rows <= 128 else 256
 
 
-def gemm_branches(w_rows, *, act=0, out_fp32=False, bn=0, vec=True, rowvec=False, residual=False, blend=False):
-    b = [f"gemm bn{gemm_bn(w_rows, act == 2, bn)}" + (" forced" if bn else " auto")]
+def gemm_operand_path(*, vec, out_fp32=False, geglu=False, residual=False, blend=False, res_strides=(8, 0, 0, 0),
+                      out_dims=(1, 1, 1, 1)):
+    """True: residual / blend source come by TMA (gemm_conv_kernel<BN, bf16, kOps = true>).  The bf16 non-GEGLU
+    epilogue on the aligned path with either source present, unless a row dim of the output has a negative residual
+    stride, or stride 0 with more than one point (a broadcast, which a tensor map cannot express)"""
+    if not (vec and not out_fp32 and not geglu and (residual or blend)):
+        return False
+    return all(s >= 0 and not (s == 0 and d > 1) for s, d in zip(res_strides, out_dims))
+
+
+def gemm_branches(w_rows, *, act=0, out_fp32=False, bn=0, vec=True, rowvec=False, residual=False, blend=False,
+                  res_strides=(8, 0, 0, 0), out_dims=(1, 1, 1, 1)):
+    """res_strides / out_dims: ca_gemm's res_strides and out_dims (the defaults: a plain row-major source)"""
+    n_tile = gemm_bn(w_rows, act == 2, bn)
+    b = [f"gemm bn{n_tile}" + (" forced" if bn else " auto")]
     if out_fp32:
         b.append("gemm epilogue f32")
     elif act == 2:
@@ -49,7 +68,32 @@ def gemm_branches(w_rows, *, act=0, out_fp32=False, bn=0, vec=True, rowvec=False
     else:
         b.append("gemm epilogue bf16")
         kind = int(rowvec) | 2 * int(residual) | 4 * int(blend)
-        b.append(f"gemm storer kind{kind} {'vec' if vec else 'elementwise'}")
+        if gemm_operand_path(vec=vec, residual=residual, blend=blend, res_strides=res_strides, out_dims=out_dims):
+            b += [f"gemm operands tma bn{n_tile}", f"gemm operands tma kind{kind}"]
+        else:
+            b.append(f"gemm storer kind{kind} {'vec' if vec else 'elementwise'}")
+            if vec and kind >= 2:
+                b.append(f"gemm operands global kind{kind} vec")
+    return b
+
+
+def attention_nwg(head_dim_pad, lq, lk):
+    """consumer warpgroups of attention_kernel (use_wg3): 3 (192-row query tiles) for head dim 64 with more than one KV
+    tile, unless their padding exceeds the 128-row tiles' by more than lq / 25"""
+    if head_dim_pad != 64 or lk <= 128:
+        return 2
+    pad192 = -lq % 192
+    pad128 = -lq % 128
+    return 3 if 25 * (pad192 - pad128) <= lq else 2
+
+
+def attention_branches(head_dim_pad, lq, lk, kv_div):
+    dq, nwg, div = head_dim_pad // 64, attention_nwg(head_dim_pad, lq, lk), "1" if kv_div == 1 else ">1"
+    b = [f"attention DQ{dq} kv_div{div}"]
+    if nwg == 3:
+        b.append(f"attention DQ{dq} NWG3 kv_div{div}")
+    else:
+        b.append(f"attention DQ{dq} NWG2 {'multi-tile' if lk > 128 else 'single-tile'}")
     return b
 
 
@@ -68,12 +112,87 @@ def expected_branches():
     b = {f"gemm bn{n} {m}" for n in (64, 128, 160, 256) for m in ("auto", "forced")}
     b |= {f"gemm storer kind{k} {d}" for k in range(8) for d in ("vec", "elementwise")}
     b |= {"gemm epilogue f32", "gemm epilogue geglu", "gemm epilogue bf16"}
+    b |= {f"gemm operands tma bn{n}" for n in (64, 128, 160, 256)} | {f"gemm operands tma kind{k}" for k in range(2, 8)}
+    b |= {f"gemm operands global kind{k} vec" for k in range(2, 8)}
     b |= set(LAYERNORM_VARIANTS) | {"layernorm in place"}
     b |= {f"attention DQ{d} kv_div{k}" for d in (1, 2, 3) for k in ("1", ">1")}
+    b |= {"attention DQ1 NWG3 kv_div1", "attention DQ1 NWG3 kv_div>1"}
+    b |= {f"attention DQ{d} NWG2 {t}" for d in (1, 2, 3) for t in ("multi-tile", "single-tile")}
     b |= {"temporal_attention SEQ16", "temporal_attention SEQ32"}
     b |= {f"gn_apply silu{s} up{u}" for s in (0, 1) for u in (0, 1)}
     b |= {"nchw_to_nhwc src bf16", "nchw_to_nhwc src fp32", "nhwc_to_nchw dst bf16", "nhwc_to_nchw dst fp32"}
     return b
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the dispatch as launched: every choice above that is a template argument shows in the kernel's name
+# ----------------------------------------------------------------------------------------------------------------------
+_KERNELS = ("attention_kernel", "gemm_conv_kernel", "layernorm_kernel", "temporal_attention_tc_kernel",
+            "gn_apply_kernel", "nchw_to_nhwc_kernel", "nhwc_to_nchw_kernel")
+_DEMANGLED = re.compile(r"\b(" + "|".join(_KERNELS) + r")<([^<>()]*)>")
+_MANGLED = re.compile(r"\d+(" + "|".join(_KERNELS) + r")I((?:L[ib]\d+E|f|14__nv_bfloat16)+)E")
+_MANGLED_ARG = re.compile(r"L[ib](\d+)E|(f)|(14__nv_bfloat16)")
+_EPILOGUES = {0: "bf16", 1: "geglu", 2: "f32"}  # GemmEpilogue
+
+
+def kernel_instantiation(name):
+    """kernel name as the profiler reports it (demangled, or an Itanium-mangled symbol) -> (kernel, template arguments
+    as ints / 'bf16' / 'fp32'), or None for a kernel without dispatch in its name"""
+    m = _DEMANGLED.search(name)
+    if m:
+        args = []
+        for a in (x.strip() for x in m.group(2).split(",")):
+            a = re.sub(r"^\((?:int|bool)\)", "", a)
+            args.append({"true": 1, "false": 0, "float": "fp32", "__nv_bfloat16": "bf16"}.get(a) if not a.isdigit()
+                        else int(a))
+        return m.group(1), tuple(args)
+    m = _MANGLED.search(name)
+    if m:
+        args = tuple(int(i) if i else "fp32" if f else "bf16" for i, f, _ in _MANGLED_ARG.findall(m.group(2)))
+        return m.group(1), args
+    return None
+
+
+def kernel_labels(name):
+    """the branch labels one launched kernel shows (the name-visible part of the labels the cases predict)"""
+    inst = kernel_instantiation(name)
+    if inst is None:
+        return set()
+    k, a = inst
+    if k == "attention_kernel":
+        return {f"attention DQ{a[0]}", f"attention DQ{a[0]} NWG{a[1]}"}
+    if k == "gemm_conv_kernel":
+        b = {f"gemm bn{a[0]}", f"gemm epilogue {_EPILOGUES[a[1]]}"}
+        return b | {f"gemm kOps{a[2]}"} if a[1] == 0 else b  # kOps exists for the plain bf16 epilogue only
+    if k == "layernorm_kernel":
+        return {f"layernorm NV{a[0]} L{a[1]} RV{a[2]}"}
+    if k == "temporal_attention_tc_kernel":
+        return {f"temporal_attention SEQ{a[0]}"}
+    if k == "gn_apply_kernel":
+        return {f"gn_apply silu{a[0]} up{a[1]}"}
+    return {f"nchw_to_nhwc src {a[0]}" if k == "nchw_to_nhwc_kernel" else f"nhwc_to_nchw dst {a[0]}"}
+
+
+def visible_parts(branch):
+    """the kernel_labels a predicted branch implies; empty for one decided at run time inside one instantiation (the
+    storer kind, vectorised vs element-wise draining, kv_batch_div, the KV tile count, LayerNorm in place)"""
+    m = re.fullmatch(r"gemm bn(\d+) (auto|forced)", branch)
+    if m:
+        return {f"gemm bn{m.group(1)}"}
+    if branch.startswith("gemm epilogue "):
+        return {branch}
+    if branch.startswith("gemm storer ") or branch.startswith("gemm operands global "):
+        return {"gemm kOps0"}
+    m = re.fullmatch(r"gemm operands tma (bn(\d+)|kind\d)", branch)
+    if m:
+        return {"gemm kOps1"} | ({f"gemm bn{m.group(2)}"} if m.group(2) else set())
+    m = re.fullmatch(r"attention DQ(\d)( NWG(\d))?.*", branch)
+    if m:
+        return {f"attention DQ{m.group(1)}"} | ({f"attention DQ{m.group(1)} NWG{m.group(3)}"} if m.group(2) else set())
+    if re.fullmatch(r"layernorm NV\d+ L\d+ RV\d|temporal_attention SEQ\d+|gn_apply silu\d up\d|"
+                    r"nchw_to_nhwc src \w+|nhwc_to_nchw dst \w+", branch):
+        return {branch}
+    return set()
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -172,6 +291,101 @@ def _gemm_cases(s):
     return out
 
 
+def _epilogue_linear(label, m, k, n, kind, *, bn=0, rpv=40, res_pad=0, broadcast=False, out_over_res=False):
+    """a bf16 linear with storer kind `kind` (1 row vector, 2 residual, 4 blend source).  res_pad: residual and blend
+    source as 16-byte-aligned views with row stride n + res_pad (ops.linear reads both with the residual's stride);
+    broadcast: both are one row expanded along M (stride 0); out_over_res: the output written over the residual"""
+    rv, res, bl = bool(kind & 1), bool(kind & 2), bool(kind & 4)
+
+    def make(dev, g):
+        kw = dict(x=_rn(g, (m, k), dev), w=_rn(g, (n, k), dev, k ** -0.5), bias=_rn(g, (n,), dev, 0.5).float(), bn=bn)
+        if rv:
+            kw["rowvec"], kw["rows_per_vec"] = _rn(g, (m // rpv, n), dev), rpv
+
+        def source():
+            if broadcast:
+                return _rn(g, (1, n), dev).expand(m, n)
+            t = _rn(g, (m, n), dev)
+            return _slot(t, 0, res_pad) if res_pad else t
+        if res:
+            kw["residual"] = source()
+        if bl:
+            kw["blend_src"] = source()
+            kw["blend_alpha"] = torch.tensor([0.3], device=dev).to(BF16).float()
+        if out_over_res:
+            kw["out"] = kw["residual"]
+        return kw
+    stride = 0 if broadcast else n + res_pad  # ops.linear's res_strides and out_dims
+    rs, dims = ((stride, rpv * stride, 0, 0), (rpv, m // rpv, 1, 1)) if rv else ((stride, 0, 0, 0), (m, 1, 1, 1))
+    return Case("linear", label, tuple(gemm_branches(n, bn=bn, rowvec=rv, residual=res, blend=bl, res_strides=rs,
+                                                     out_dims=dims)), make)
+
+
+def _gemm_operand_cases():
+    """the bf16 epilogue's residual / blend source by TMA (kOps): every N tile automatic and forced, partial 32-column
+    slabs (n_out 8, 24, 40, 168, 200), M not a multiple of 128 with more tiles than SMs, strided sources, row vectors
+    over fewer than 128 rows (the 2-D box), the output written over the residual, convolutions with boxes reaching past
+    the image; and the broadcast sources (stride 0 along M) that keep the per-chunk global loads"""
+    out = []
+    for i, n in enumerate((8, 24, 40, 96, 168, 320)):  # automatic N tile 64, 64, 64, 128, 256, 160
+        kind = 2 + i
+        out.append(_epilogue_linear(f"linear ops n{n} kind{kind}", 200, 64, n, kind))
+    for bn in (64, 128, 160, 256):
+        for kind in range(2, 8):
+            out.append(_epilogue_linear(f"linear ops n200 bn{bn} kind{kind}", 200, 64, 200, kind, bn=bn))
+    out.append(_epilogue_linear("linear ops m4500 n200 bn64 kind6", 4500, 64, 200, 6, bn=64))  # 144 tiles
+    out.append(_epilogue_linear("linear ops m4500 n320 bn64 kind7 rpv180", 4500, 64, 320, 7, bn=64, rpv=180))
+    out.append(_epilogue_linear("linear ops m9000 n512 kind2", 9000, 64, 512, 2))  # BN 256: 142 tiles
+    for n, bn, kind in ((96, 0, 2), (96, 0, 4), (96, 0, 6), (200, 160, 7)):
+        out.append(_epilogue_linear(f"linear ops n{n} bn{bn} kind{kind} source stride n+8", 200, 64, n, kind, bn=bn,
+                                    res_pad=8))
+    for kind in (3, 7):
+        out.append(_epilogue_linear(f"linear ops m192 n96 kind{kind} rpv48", 192, 64, 96, kind, rpv=48))
+    for bn, kind in ((64, 2), (128, 2), (160, 6), (256, 3)):
+        out.append(_epilogue_linear(f"linear ops n200 bn{bn} kind{kind} out over residual", 200, 64, 200, kind, bn=bn,
+                                    out_over_res=True))
+    for kind, n in zip(range(2, 8), (40, 96, 320, 512, 40, 320)):  # automatic N tile 64, 128, 160, 256, 64, 160
+        out.append(_epilogue_linear(f"linear broadcast sources m192 n{n} kind{kind}", 192, 64, n, kind, rpv=64,
+                                    broadcast=True))
+    from ctrl_adapter_b200.ops import pack_conv_weight
+
+    def conv(n, h, w, c0, c1, cout, kind):
+        def make(dev, g):
+            kw = dict(x=_rn(g, (n, h, w, c0), dev), bias=_rn(g, (cout,), dev, 0.5).float(),
+                      w_packed=pack_conv_weight(_rn(g, (cout, c0 + c1, 3, 3), dev, (c0 + c1) ** -0.5 / 3)))
+            if c1:
+                kw["x2"] = _rn(g, (n, h, w, c1), dev)
+            if kind & 1:
+                kw["rowvec"] = _rn(g, (n, cout), dev)
+            if kind & 2:
+                kw["residual"] = _rn(g, (n, h, w, cout), dev)
+            if kind & 4:
+                kw["blend_src"] = _rn(g, (n, h, w, cout), dev)
+                kw["blend_alpha"] = torch.tensor([0.7], device=dev).to(BF16).float()
+            return kw
+        out.append(Case("conv2d", f"conv3x3 n{n} {h}x{w} c{c0}+{c1} cout{cout} kind{kind}",
+                        tuple(gemm_branches(cout, rowvec=bool(kind & 1), residual=bool(kind & 2),
+                                            blend=bool(kind & 4))), make))
+    conv(2, 6, 10, 64, 0, 40, 2)
+    conv(2, 6, 10, 64, 0, 40, 7)
+    conv(2, 5, 7, 64, 32, 96, 6)
+    conv(1, 6, 10, 64, 0, 40, 3)
+    conv(1, 5, 7, 64, 32, 168, 6)
+    for frames, kind in ((5, 6), (3, 7)):
+        def make_t(dev, g, frames=frames, kind=kind):
+            c, cout = 64, 96
+            kw = dict(x=_rn(g, (2 * frames, 3, 5, c), dev), bias=_rn(g, (cout,), dev, 0.5).float(), frames=frames,
+                      w_packed=pack_conv_weight(_rn(g, (cout, c, 3, 1, 1), dev, (3 * c) ** -0.5)),
+                      residual=_rn(g, (2 * frames, 3, 5, cout), dev), blend_src=_rn(g, (2 * frames, 3, 5, cout), dev),
+                      blend_alpha=torch.tensor([0.4], device=dev).to(BF16).float())
+            if kind & 1:
+                kw["rowvec"] = _rn(g, (2 * frames, cout), dev)
+            return kw
+        out.append(Case("temporal_conv", f"temporal_conv frames{frames} kind{kind}",
+                        tuple(gemm_branches(96, rowvec=bool(kind & 1), residual=True, blend=True)), make_t))
+    return out
+
+
 def _norm_cases(s):
     out = []
     # LayerNorm: one width per (NV, L) instantiation, 8 <= c <= 2048, with and without the row vector
@@ -215,6 +429,49 @@ def _norm_cases(s):
     return out
 
 
+def _attention_tile_cases():
+    """KV rings of more than one tile and the 192-row query tiles (attention_nwg) under guard bands: head dim 64 on
+    both sides of every flip of the tile rule, lk 129 (a 1-key last tile) to 1300 (11 tiles through the 4-slot ring),
+    shared contexts, fused-QKV views (row stride 3 C), an output view with gap columns, head dims 128 and 192.  peaks:
+    (query row, key) pairs whose query is 3x that key, so the row's logits peak there ~20 above the rest: in the
+    ragged last KV tile (every earlier tile's running max and sum must be rescaled) or in the first"""
+    out = []
+
+    def case(dp, lq, lk, *, b=1, heads=2, div=1, fused=False, out_gap=0, peaks=()):
+        def make(dev, g):
+            d, c = dp - 16, heads * dp  # zero-padded head dim, as the modules pack it
+
+            def padded(bb, ll):
+                t = torch.zeros(bb, ll, heads, dp)
+                t[..., :d] = torch.randn(bb, ll, heads, d, generator=g)
+                return t
+            q, k, v = padded(b, lq), padded(b // div, lk), padded(b // div, lk)
+            for row, key in peaks:
+                q[:, row] = 3.0 * k[torch.arange(b) // div, key]
+            if fused:  # Q, K, V as column views of one [b, l, 3 C] projection
+                qkv = torch.cat([t.reshape(b, lq, c) for t in (q, k, v)], dim=2).to(BF16).to(dev)
+                kw = dict(q=qkv[..., :c], k=qkv[..., c:2 * c], v=qkv[..., 2 * c:])
+            else:
+                kw = {n: t.reshape(t.shape[0], t.shape[1], c).to(BF16).to(dev) for n, t in zip("qkv", (q, k, v))}
+            if out_gap:
+                kw["out"] = torch.zeros(b, lq, c + out_gap, dtype=BF16, device=dev)[..., :c]
+            return dict(kw, heads=heads, head_dim_pad=dp, scale=d ** -0.5, kv_batch_div=div)
+        tags = " fused-qkv" * fused + f" out gap{out_gap}" * bool(out_gap) + f" peaks{list(peaks)}" * bool(peaks)
+        out.append(Case("attention", f"attention dp{dp} b{b} lq{lq} lk{lk} kv_div{div}{tags}",
+                        tuple(attention_branches(dp, lq, lk, div)), make))
+    for lq, lk in ((1, 128), (1, 129), (128, 257), (129, 257), (144, 1300), (191, 129), (192, 128), (192, 129),
+                   (193, 257), (576, 1300), (577, 257), (1599, 129), (1600, 257)):
+        case(64, lq, lk)
+    case(64, 192, 300, b=4, div=2, peaks=((0, 299), (191, 0)))
+    case(64, 300, 300, fused=True, peaks=((5, 299), (77, 3)))
+    case(64, 577, 577, fused=True)
+    case(64, 384, 300, out_gap=16)
+    case(64, 193, 1300, peaks=((0, 1299), (192, 0)))
+    case(128, 300, 257, out_gap=16, peaks=((1, 256), (299, 2)))
+    case(192, 200, 300, b=4, div=2, peaks=((3, 299), (150, 0)))
+    return out
+
+
 def _attention_cases(s):
     out = []
     for dp in (64, 128, 192):
@@ -229,8 +486,9 @@ def _attention_cases(s):
                     return t.reshape(bb, ll, heads * dp).to(BF16).to(dev)
                 return dict(q=padded(b, lq), k=padded(b // div, lk), v=padded(b // div, lk), heads=heads,
                             head_dim_pad=dp, scale=d ** -0.5, kv_batch_div=div)
-            out.append(Case("attention", f"attention dp{dp} kv_div{div}",
-                            (f"attention DQ{dp // 64} kv_div{'1' if div == 1 else '>1'}",), make))
+            out.append(Case("attention", f"attention dp{dp} kv_div{div}", tuple(attention_branches(dp, lq, lk, div)),
+                            make))
+    out += _attention_tile_cases()
     hw = 11 if s else 37
     for frames in range(1, 33):  # every frame count either SEQ instantiation takes
         def make(dev, g, frames=frames):
@@ -353,8 +611,8 @@ def _scheduler_cases(s):
 
 def cases(small=False, seed=0):
     rng = random.Random(seed)
-    return (_gemm_cases(small) + _norm_cases(small) + _attention_cases(small) + _small_op_cases(small, rng) +
-            _scheduler_cases(small))
+    return (_gemm_cases(small) + _gemm_operand_cases() + _norm_cases(small) + _attention_cases(small) +
+            _small_op_cases(small, rng) + _scheduler_cases(small))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -541,19 +799,78 @@ def layernorm_in_place(a, device):
     return y, y_sum
 
 
-def run_cases(cs, device, recorder):
-    """every case: `ops` calls through the (entered) recorder, direct C calls checked here.
+class KernelTrace:
+    """with KernelTrace() as tr, Recorder() as rec: -- wraps the `ops` entry points before the recorder wraps them, so
+    that the first launch after arm() (the recorder's in-step launch, not its re-runs or replay) runs under
+    torch.profiler, kernel trace only (ProfilerActivity.CUDA: no hardware counters).  tr.names: the CUDA events of that
+    launch (None: nothing ran under the trace)."""
+
+    def __init__(self):
+        self.armed, self.names, self._saved = False, None, {}
+
+    def __enter__(self):
+        from ctrl_adapter_b200 import ops
+        from tests import launch_checks as lc
+        for name in lc.OPS:
+            fn = self._saved[name] = getattr(ops, name)
+            setattr(ops, name, self._wrap(fn))
+        return self
+
+    def __exit__(self, *exc):
+        from ctrl_adapter_b200 import ops
+        for name, fn in self._saved.items():
+            setattr(ops, name, fn)
+        self._saved = {}
+        return False
+
+    def arm(self):
+        self.armed, self.names = True, None
+
+    def _wrap(self, fn):
+        def traced(*args, **kw):
+            if not self.armed:
+                return fn(*args, **kw)
+            return self.run(lambda: fn(*args, **kw))
+        return traced
+
+    def run(self, call):
+        from torch.autograd import DeviceType
+        from torch.profiler import ProfilerActivity, profile
+        self.armed = False
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            # margins on both sides of the launch: a trace now and then comes back without the launch's device events
+            # (3 of 319 traces in one sweep without them, 1 of 319 with them; run_cases then traces the case again)
+            time.sleep(0.005)
+            ret = call()
+            torch.cuda.synchronize()
+            time.sleep(0.005)
+        self.names = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
+        return ret
+
+
+def run_cases(cs, device, recorder, trace=None):
+    """every case: `ops` calls through the (entered) recorder, direct C calls checked here.  trace: an entered
+    KernelTrace; the names of the kernels each case's first launch ran go to trace.seen[case label].
     -> {case label: (op, rows checked, worst err/tol, ok, why)}"""
     from ctrl_adapter_b200 import ops
     from tests import kernel_checks as kc
     from tests import launch_checks as lc
     out = {}
+    if trace is not None:
+        trace.seen = {}
     for i, case in enumerate(cs):
         g = torch.Generator().manual_seed(1000 + i)
         kw = case.make(device, g)
+        if trace is not None:
+            trace.arm()
         if case.op.startswith("lib:"):
             pre = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in kw.items()}
-            y, ys = layernorm_in_place(kw, device)
+            if trace is None:
+                y, ys = layernorm_in_place(kw, device)
+            else:
+                y, ys = trace.run(lambda: layernorm_in_place(kw, device))
+                _retrace(trace, case, i, device)
             kc._sync()
             row = lc.Row(case.op, ())
             try:
@@ -566,11 +883,30 @@ def run_cases(cs, device, recorder):
         before = set(recorder.rows)
         getattr(ops, case.op)(**kw)
         kc._sync()
+        if trace is not None:
+            _retrace(trace, case, i, device)
         new = [recorder.rows[k] for k in recorder.rows if k not in before]
         if not new:  # the same configuration as an earlier case: that row stands for it
             new = [recorder.rows[lc.config_key(case.op, _bound(case.op, kw))]]
         out[case.label] = (case.op, new)
     return out
+
+
+def _retrace(trace, case, i, device):
+    """trace.seen[case label] = the trace's CUDA events.  A trace that came back without any: the case launched again
+    on fresh inputs (the same configuration, its first launch already checked) under a new trace, at most twice"""
+    from ctrl_adapter_b200 import ops
+    for _ in range(2):
+        if trace.names:
+            break
+        kw = case.make(device, torch.Generator().manual_seed(1000 + i))
+        trace.arm()
+        if case.op.startswith("lib:"):
+            trace.run(lambda: layernorm_in_place(kw, device))
+        else:
+            getattr(ops, case.op)(**kw)
+        torch.cuda.synchronize()
+    trace.seen[case.label] = trace.names
 
 
 def _bound(op, kw):
@@ -599,3 +935,37 @@ def summary(cs, results):
 
 def failures(results):
     return [(label, r) for label, (_, rows) in results.items() for r in rows if not r.ok]
+
+
+def observed_dispatch(cs, seen):
+    """cases vs the kernels their first launch ran (seen: {case label: CUDA event names}).
+    -> (problems, reached, instantiations): a problem per case whose trace holds no CUDA event, or whose predicted
+    name-visible labels are not exactly those of its kernels; the branches reached, each counted only where its
+    name-visible part was observed; {kernel<template arguments>: number of cases}"""
+    problems, reached, inst = [], set(), {}
+    for case in cs:
+        names = seen.get(case.label)
+        if not names:
+            problems.append(f"{case.label}: torch.profiler recorded no CUDA kernel event for its first launch")
+            continue
+        observed = set().union(*(kernel_labels(n) for n in names))
+        predicted = set().union(*(visible_parts(b) for b in case.branches))
+        if predicted != observed:
+            problems.append(f"{case.label}: predicted {sorted(predicted - observed)}, observed {sorted(observed - predicted)}")
+        reached |= {b for b in case.branches if visible_parts(b) <= observed}
+        for k in {kernel_instantiation(n) for n in names} - {None}:
+            key = f"{k[0]}<{', '.join(map(str, k[1]))}>"
+            inst[key] = inst.get(key, 0) + 1
+    return problems, reached, inst
+
+
+def dispatch_summary(reached, inst):
+    """the kernel instantiations observed, and the expected branches that are run-time switches (predicted only)"""
+    lines = [f"\n{'observed instantiation':<44} {'cases':>6}"]
+    lines += [f"{k:<44} {n:>6}" for k, n in sorted(inst.items())]
+    predicted = sorted(b for b in expected_branches() & reached if not visible_parts(b))
+    partly = sorted(b for b in expected_branches() & reached if visible_parts(b) and visible_parts(b) != {b})
+    lines.append(f"\nbranches observed in kernel names: {len(expected_branches() & reached) - len(predicted) - len(partly)}")
+    lines.append(f"observed in part (the instantiation; the rest a run-time switch): {', '.join(partly)}")
+    lines.append(f"predicted only (run-time switches): {', '.join(predicted)}")
+    return "\n".join(lines)

@@ -272,6 +272,15 @@ def _view_on(storage, t, byte_off):
     return torch.empty(0, dtype=t.dtype, device=t.device).set_(storage, byte_off // t.element_size(), t.shape, t.stride())
 
 
+def _distinct(t):
+    """t without the repeats of a broadcast (an expanded dim of stride 0 narrowed to its first point): the same
+    elements, each once, so that it can be written"""
+    for d, (n, s) in enumerate(zip(t.shape, t.stride())):
+        if s == 0 and n > 1:
+            t = t.narrow(d, 0, 1)
+    return t
+
+
 def _dense(views, lo, hi):
     """the contiguous views among `views` cover the byte range [lo, hi) with no gap"""
     spans = sorted(_byte_range(t) for t in views if t.is_contiguous())
@@ -316,7 +325,7 @@ class _Clone:
             shift = GUARD + (st.data_ptr() + lo - buf.data_ptr()) % 16
             self.bufs[key] = (buf, shift)
             for t in self.views[key]:
-                self.view(t).copy_(t)
+                _distinct(self.view(t)).copy_(_distinct(t))
 
     def view(self, t):
         buf, shift = self.bufs[_storage_key(t)]

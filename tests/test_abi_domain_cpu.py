@@ -4,7 +4,9 @@ outside the header's domain.
     recorder of tests/launch_checks.py, and the cases reach every predicted dispatch branch;
 (b) each deliberately wrong variant of an emulated op below fails at least one case (printed with -s);
 (c) for every constraint of abi_domain.DOMAIN, the real library (ctypes, no GPU) lets the last value inside through
-    validation and rejects the first value outside with CA_ERR_INVALID and a message naming the argument."""
+    validation and rejects the first value outside with CA_ERR_INVALID and a message naming the argument;
+(d) the restated 192-row attention tile rule matches its boundary table, and the kernel-name parser of the GPU sweep
+    reads fixed demangled and mangled names."""
 import pytest
 import torch
 
@@ -109,7 +111,74 @@ def _router_mask_first_8(logits, mask):
     return emu.router_weights(logits, mask)
 
 
+def _attention_tiled(q, k, v, heads, head_dim_pad, scale, out=None, kv_batch_div=1, *, rescale=True,
+                     ragged_tail=True):
+    """online softmax over 128-key tiles.  rescale=False: the running sum and output are not rescaled when a later tile
+    raises the row max; ragged_tail=False: with more than one tile, the keys of a partial last tile are dropped"""
+    b, lq, _ = q.shape
+    lk = k.shape[1]
+    qh = q.float().reshape(b, lq, heads, head_dim_pad).permute(0, 2, 1, 3)
+    kb = torch.arange(b) // kv_batch_div
+    kh, vh = (t.float().reshape(t.shape[0], lk, heads, head_dim_pad).permute(0, 2, 1, 3)[kb] for t in (k, v))
+    if not ragged_tail and lk > 128:
+        kh, vh = kh[:, :, :lk // 128 * 128], vh[:, :, :lk // 128 * 128]
+    m = torch.full((b, heads, lq, 1), -float("inf"))
+    l, o = torch.zeros(b, heads, lq, 1), torch.zeros(b, heads, lq, head_dim_pad)
+    for j in range(0, kh.shape[2], 128):
+        s = qh @ kh[:, :, j:j + 128].transpose(-1, -2) * scale
+        m_new = torch.maximum(m, s.amax(-1, keepdim=True))
+        p = torch.exp(s - m_new)
+        corr = torch.exp(m - m_new) if rescale else torch.ones_like(m)
+        l, o, m = l * corr + p.sum(-1, keepdim=True), o * corr + p @ vh[:, :, j:j + 128], m_new
+    y = (o / l).permute(0, 2, 1, 3).reshape(b, lq, heads * head_dim_pad).to(BF16)
+    if out is not None:
+        out.copy_(y)
+        return out
+    return y
+
+
+def _attention_no_rescale(*args, **kw):
+    return _attention_tiled(*args, **kw, rescale=False)
+
+
+def _attention_drops_ragged_tail(*args, **kw):
+    return _attention_tiled(*args, **kw, ragged_tail=False)
+
+
+def _read_as(t, shape, stride):
+    """t's storage read from t's first element with another shape / stride; elements past the storage are NaN (a guard
+    band)"""
+    flat = torch.empty(0, dtype=t.dtype).set_(t.untyped_storage(), t.storage_offset(),
+                                                (t.untyped_storage().nbytes() // t.element_size() - t.storage_offset(),))
+    idx = sum(torch.arange(n).reshape([-1 if i == d else 1 for i in range(len(shape))]) * s
+              for d, (n, s) in enumerate(zip(shape, stride)))
+    nan = torch.full((), float("nan"), dtype=t.dtype)
+    return torch.where(idx < flat.numel(), flat[idx.clamp(max=flat.numel() - 1)], nan)
+
+
+def _linear_residual_output_stride(x, w, bias=None, *, residual=None, out=None, **kw):
+    """the residual (and blend source) read with the output's row stride instead of its own"""
+    m, n = x.shape[0], w.shape[0]
+    ostride = (n, 1) if out is None else out.stride()
+    if residual is not None and residual.stride() != ostride:
+        residual = _read_as(residual, (m, n), ostride)
+        if kw.get("blend_src") is not None:
+            kw["blend_src"] = _read_as(kw["blend_src"], (m, n), ostride)
+    return emu.linear(x, w, bias, residual=residual, out=out, **kw)
+
+
+def _linear_broadcast_as_contiguous(x, w, bias=None, *, residual=None, blend_src=None, **kw):
+    """a residual / blend source broadcast along M (stride 0) read as if it were a contiguous [M, N]"""
+    fix = lambda t: t if t is None or t.stride(0) != 0 else _read_as(t, t.shape, (t.shape[1], 1))  # noqa: E731
+    return emu.linear(x, w, bias, residual=fix(residual), blend_src=fix(blend_src), **kw)
+
+
 VARIANTS = {
+    "attention: running sum and output not rescaled when a later KV tile raises the max":
+        {"attention": _attention_no_rescale},
+    "attention: the keys of a ragged last KV tile dropped": {"attention": _attention_drops_ragged_tail},
+    "linear: residual read with the output's row stride": {"linear": _linear_residual_output_stride},
+    "linear: broadcast residual / blend source read as contiguous": {"linear": _linear_broadcast_as_contiguous},
     "silu: reads one vector past its end": {"silu": _silu_reads_past_end},
     "linear: residual read from the stride gap": {"linear": _linear_residual_gap},
     "group_norm: groups ignored": {"group_norm": _gn_ignores_groups},
@@ -126,6 +195,60 @@ def test_sweep_catches_wrong_variant(variant):
     print(f"\n{variant}: caught by " + ("; ".join(f"{label} [{r.where}] {r.why[0][:80]}" for label, r in bad[:2])
                                        or "NOTHING"))
     assert bad, f"no case notices: {variant}"
+
+
+# ---- (d) the restated dispatch rules and the kernel-name parser of the GPU sweep ----
+# (lq, lk, head_dim_pad, 192-row tiles?): the boundaries of ca_attention's use_wg3.  1600 is where 25 (pad192 - pad128)
+# == lq: the rule's <= decides it.
+NWG_TABLE = ([(lq, 257, 64, False) for lq in (1, 64, 127, 128)] +
+             [(129, 257, 64, True), (192, 257, 64, True), (193, 257, 64, False), (256, 257, 64, False),
+              (257, 257, 64, True), (576, 257, 64, True), (577, 257, 64, False), (1599, 257, 64, False),
+              (1600, 257, 64, True), (2880, 257, 64, True), (2881, 257, 64, False), (2944, 257, 64, False),
+              (2945, 257, 64, True), (192, 128, 64, False), (192, 129, 64, True)] +
+             [(lq, 1300, dp, False) for dp in (128, 192) for lq in (129, 192, 576, 1600, 2945, 4096)])
+
+
+def test_attention_nwg_table():
+    got = [(lq, lk, dp, ad.attention_nwg(dp, lq, lk) == 3) for lq, lk, dp, _ in NWG_TABLE]
+    assert got == NWG_TABLE
+    assert all(ad.attention_nwg(64, lq, lk) == 3 for lq in range(2945, 20000) for lk in (129, 4096))
+    assert all(ad.attention_nwg(64, lq, 128) == 2 for lq in range(1, 20000))
+
+
+KERNEL_NAMES = [
+    ("void ca::attention_kernel<1, 3>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, ca::AttnParams)",
+     {"attention DQ1", "attention DQ1 NWG3"}),
+    ("void ca::attention_kernel<3, 2>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, ca::AttnParams)",
+     {"attention DQ3", "attention DQ3 NWG2"}),
+    ("_ZN2ca16attention_kernelILi2ELi2EEEv14CUtensorMap_stS1_S1_NS_10AttnParamsE",
+     {"attention DQ2", "attention DQ2 NWG2"}),
+    ("void ca::gemm_conv_kernel<160, 0, true>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, "
+     "CUtensorMap_st, ca::GemmParams)", {"gemm bn160", "gemm epilogue bf16", "gemm kOps1"}),
+    ("void ca::gemm_conv_kernel<64, 0, false>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, "
+     "CUtensorMap_st, ca::GemmParams)", {"gemm bn64", "gemm epilogue bf16", "gemm kOps0"}),
+    ("void ca::gemm_conv_kernel<256, 1, false>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, "
+     "CUtensorMap_st, ca::GemmParams)", {"gemm bn256", "gemm epilogue geglu"}),
+    ("_ZN2ca16gemm_conv_kernelILi128ELi2ELb0EEEv14CUtensorMap_stS1_S1_S1_S1_NS_10GemmParamsE",
+     {"gemm bn128", "gemm epilogue f32"}),
+    ("void ca::layernorm_kernel<3, 16, true>(__nv_bfloat16 const*, long long, int, float, float const*, float const*, "
+     "__nv_bfloat16 const*, int, __nv_bfloat16*, __nv_bfloat16*)", {"layernorm NV3 L16 RV1"}),
+    ("void ca::temporal_attention_tc_kernel<32>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, ca::TaParams)",
+     {"temporal_attention SEQ32"}),
+    ("void ca::gn_apply_kernel<false, true>(__nv_bfloat16 const*, int, __nv_bfloat16 const*, int, int, int, int, int, "
+     "float, double const*, float const*, float const*, __nv_bfloat16*)", {"gn_apply silu0 up1"}),
+    ("void ca::nchw_to_nhwc_kernel<float>(float const*, int, long long, int, __nv_bfloat16*)",
+     {"nchw_to_nhwc src fp32"}),
+    ("_ZN2ca19nhwc_to_nchw_kernelI14__nv_bfloat16EEvPKS1_iixPT_", {"nhwc_to_nchw dst bf16"}),
+    ("void ca::gn_stats_kernel(__nv_bfloat16 const*, int, __nv_bfloat16 const*, int, int, int, double*)", set()),
+    ("void at::native::vectorized_elementwise_kernel<4, at::native::FillFunctor<float>, std::array<char*, 1ul> >"
+     "(int, at::native::FillFunctor<float>, std::array<char*, 1ul>)", set()),
+    ("Memcpy DtoD (Device -> Device)", set()),
+]
+
+
+@pytest.mark.parametrize("name,labels", KERNEL_NAMES, ids=[n[:48] for n, _ in KERNEL_NAMES])
+def test_kernel_labels(name, labels):
+    assert ad.kernel_labels(name) == labels
 
 
 # ---- (c) the library's validation at every boundary of the domain ----
