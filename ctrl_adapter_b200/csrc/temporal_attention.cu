@@ -109,21 +109,31 @@ temporal_attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const _
       s[i] = pv;
       l[(i >> 1) & 1] += pv;
     }
-    uint32_t pa[4][4];  // P is bf16 in the fused SDPA kernels of the reference path
+    // P.V with P split into two bf16 terms, P = hi + lo with hi = bf16(P), lo = bf16(P - hi): P enters with ~16
+    // significant bits instead of 8.  With P rounded to bf16 alone, rows whose probabilities are nearly equal (the
+    // frames of a clip look alike) lost their small differences to the rounding, which flattened the softmax: on the
+    // video pipelines' activations every output moved toward the mean of V by 3e-4 to 1e-3 of its distance from it.
+    uint32_t pa[4][4], pl[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
-      pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
-      pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
-      pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
-      pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const float a = s[8 * kk + 2 * m], b = s[8 * kk + 2 * m + 1];
+        const __nv_bfloat162 hi = __floats2bfloat162_rn(a, b);
+        const float2 hf = __bfloat1622float2(hi);
+        pa[kk][m] = *reinterpret_cast<const uint32_t*>(&hi);
+        pl[kk][m] = pack_bf16x2(a - hf.x, b - hf.y);
+      }
     }
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
+    for (int kk = 0; kk < 4; ++kk) {
       Wgmma<64>::rs_bt(o, pa[kk], gmma_desc_sw128(base + 2 * kTaTile + off + kk * 2048, 8192, 1024), 1);
+      Wgmma<64>::rs_bt(o, pl[kk], gmma_desc_sw128(base + 2 * kTaTile + off + kk * 2048, 8192, 1024), 1);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(o);

@@ -121,14 +121,17 @@ int ca_attention(const ca_attention_desc* d, void* cuda_stream);
 
 /*
  * GroupNorm on channels-last data, two launches: statistics (fp64 accumulation of sum / sum-of-squares per
- * (sample, group)) and apply (+SiLU, + optional 2x nearest up-sampling, + optional channel concat of two sources).
+ * (sample, group), of x minus the group's first channel at the sample's first pixel) and apply (+SiLU, + optional 2x
+ * nearest up-sampling, + optional channel concat of two sources).
  * Replaces F.group_norm + F.silu (+ Upsample2D) at model/resnet_block_2d.py:171-184,199-211,
  * model/adapter_spatial_temporal.py:254, diffusers TemporalResnetBlock / Transformer2DModel norms.
  * `sums` is a caller-provided scratch of n*groups*2 doubles (zeroed by ca_groupnorm_stats).
  * A "sample" is `rows` consecutive channel vectors (h*w, or frames*h*w for the 5-D temporal GroupNorm).
  * Constraints (both passes): 1 <= groups <= 64 dividing c0 + c1; c0, c1 multiples of 8 with 8 <= c0 + c1 <= 4096;
  * 1 <= n <= 65535; x0 (and x1 when c1 > 0) and y 16-byte aligned; stats: rows >= 1; apply: h, w >= 1, h * w < 2^30,
- * imgs_per_sample >= 1 dividing n (apply's n counts images, stats' n samples).
+ * imgs_per_sample >= 1 dividing n (apply's n counts images, stats' n samples); y must not alias x0 or x1 (apply reads
+ * each sample's first pixel back in every block), and apply must see the data stats summed, with rows = h * w *
+ * imgs_per_sample.
  */
 int ca_groupnorm_stats(const void* x0, int32_t c0, const void* x1, int32_t c1, int32_t n, int64_t rows,
                        int32_t groups, double* sums, void* cuda_stream);

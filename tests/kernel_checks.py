@@ -33,6 +33,8 @@ import sys
 import torch
 import torch.nn.functional as F
 
+from tests import error_stats as es
+
 BF16 = torch.bfloat16
 F64 = torch.float64
 RESULTS = []
@@ -55,11 +57,27 @@ def _rand(*shape, scale=1.0, seed=None, dtype=BF16):
     return (torch.randn(*shape, generator=g, device=DEVICE, dtype=torch.float32) * scale).to(dtype)
 
 
-def _report(name, out, ref, rtol, atol, extra=None, mag=None, dims=None, rows=None):
+def _report(name, out, ref, rtol, atol, extra=None, mag=None, dims=None, rows=None, units=None, gain=None, eager=None,
+            unit_shape=None, stats_ref=None):
     """mag: magnitude of the largest intermediate of a multi-step bf16 epilogue (a 1-ulp flip of an intermediate is
     1 ulp of THAT magnitude, which can be several ulps of a smaller final value after cancellation).
     dims: names of out's axes -- the record then says where the worst error / tolerance ratio is; rows: the indices the
-    first axis stands for when it holds a sample of a launch's images or batch entries."""
+    first axis stands for when it holds a sample of a launch's images or batch entries.
+    units: the axes of out that name its independent units (error_stats.BLOCKS: blocks of 4096 elements); with it the
+    record also gets the direction statistics of tests/error_stats.py (bias, gain, RMS error) and fails on them, `why`
+    naming the statistic.  gain: (axes of the gain groups, the gain's center or None, the axes its se clusters by or None
+    for `units`); eager: an eager torch op's output on the same inputs (the gain's and RMS error's yardstick);
+    unit_shape: the shape of out / ref (and eager) the axes refer to; stats_ref: the reference of the statistics when it
+    differs from ref (attention: ref rounded at the kernel's output rounding, error_stats docstring)."""
+    stats = None
+    if units is not None:
+        groups, center, gunits = gain if gain is not None else ((), None, None)
+        o, r, e = out, ref if stats_ref is None else stats_ref, eager
+        if unit_shape is not None:
+            o, r = out.reshape(unit_shape), r.reshape(unit_shape)
+            e = None if eager is None else eager.reshape(unit_shape)
+        at = atol.reshape(unit_shape) if unit_shape is not None and torch.is_tensor(atol) and atol.dim() else atol
+        stats = es.direction(o, r, at, units=units, gain_groups=groups, gain_units=gunits, center=center, eager=e)
     out = out.float()
     ref = ref.float()
     assert out.shape == ref.shape, f"{name}: shape {tuple(out.shape)} vs {tuple(ref.shape)}"
@@ -90,8 +108,20 @@ def _report(name, out, ref, rtol, atol, extra=None, mag=None, dims=None, rows=No
         rec["where"] = where
     if extra:
         rec.update(extra)
+    _add_direction(rec, stats)
     RESULTS.append(rec)
     return rec
+
+
+def _add_direction(rec, stats):
+    """the direction statistics' fields into a record; their failure fails it, `why` naming the statistic"""
+    if stats is None:
+        return
+    ok, why = stats.pop("ok"), stats.pop("why")
+    rec.update(stats)
+    if not ok:
+        rec["ok"] = False
+        rec["why"] = "; ".join(w for w in (rec.get("why"), why) if w)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -493,13 +523,19 @@ def _attn_verdict(name, q, k, v, kv_idx, scale, out, rows=None):
     wb, wh = divmod(int(err_bh.argmax()), err_bh.shape[1])
     rb, rh = divmod(int(ratio.argmax()), ratio.shape[1])
     lb = (lambda i: i) if rows is None else (lambda i: int(rows[i]))
-    rec = _report(name, out, ref, 2e-2, 2e-3, dims=("b", "q", "h", "d"), rows=rows, extra={
+    # gain per (batch, head) about the mean of V over the keys: a wrong softmax temperature moves every output of a row
+    # toward or away from it; torch's bf16 SDPA is the yardstick of the gain and of the RMS error per (batch, head)
+    vmean = v.to(F64)[kv_idx].mean(dim=1, keepdim=True)
+    sd = sd.permute(0, 2, 1, 3)
+    rec = _report(name, out, ref, 2e-2, 2e-3, dims=("b", "q", "h", "d"), rows=rows, units=(0, 1, 2),
+                  gain=((0, 2), vmean, None), eager=sd, stats_ref=_r64(ref), extra={
         "sdpa_bf16_max_err": float(sd_bh.max()), "worst_bh": f"b{lb(wb)}h{wh}", "worst_bh_err": float(err_bh[wb, wh]),
         "worst_bh_sdpa_err": float(sd_bh[wb, wh]), "max_bh_err_over_2x_sdpa": float(ratio[rb, rh]),
         "max_ratio_bh": f"b{lb(rb)}h{rh}"})
     if float(ratio.max()) > 1.0:
         rec["ok"] = False
-        rec["why"] = f"(batch, head) b{lb(rb)}h{rh}: error larger than 2x torch bf16 SDPA"
+        rec["why"] = "; ".join(w for w in (f"(batch, head) b{lb(rb)}h{rh}: error larger than 2x torch bf16 SDPA",
+                                            rec.get("why")) if w)
     return rec
 
 
@@ -564,8 +600,16 @@ def temporal_attention_verdict(name, q, k, v, clips, frames, hw, heads, scale, o
     out = out.reshape(ref.shape)
     err_f = (out.to(F64) - ref).abs().amax(dim=(0, 2, 3))  # worst error per frame
     wf = int(err_f.argmax())
+    # units: the (clip, pixel, head) sequences; gain about each sequence's mean of V over the frames; yardstick: torch's
+    # bf16 SDPA on the same sequences
+    vmean = seq(v).mean(dim=3, keepdim=True).permute(0, 3, 1, 2, 4)
+
+    def seq16(t):
+        return t.reshape(clips, frames, hw, heads, 64).permute(0, 2, 3, 1, 4)
+    sd = F.scaled_dot_product_attention(seq16(q), seq16(k), seq16(v), scale=scale).permute(0, 3, 1, 2, 4)
     return _report(name, out, ref, 2e-2, 6e-3, {"worst_frame": wf, "worst_frame_err": float(err_f[wf])},
-                   dims=("clip", "frame", "pixel", "ch"))
+                   dims=("clip", "frame", "pixel", "ch"), units=(0, 2, 3), gain=((), vmean, None), eager=sd,
+                   unit_shape=(clips, frames, hw, heads, 64), stats_ref=_r64(ref))
 
 
 EPILOGUES = ("bias", "bias_silu", "bias_scale", "bias_scale_res", "rowvec", "bias_res", "rowvec_res", "bias_res_blend",
@@ -679,7 +723,8 @@ def _f32_epilogue_verdict(name, pre, out, a, rv, dims, rows=None):
     if a["residual"] is not None:
         v = v + a["residual"].to(F64)
         mag = torch.maximum(mag, v.abs())
-    return _report(name, out, v, 2 ** -7 if rounded else 2 ** -20, 1e-6, mag=mag, dims=dims, rows=rows)
+    return _report(name, out, v, 2 ** -7 if rounded else 2 ** -20, 1e-6, mag=mag, dims=dims, rows=rows,
+                   units=tuple(range(out.dim() - 1)))
 
 
 def _sum_floor(abs_sum):
@@ -730,27 +775,27 @@ def linear_verdict(name, a, out, rerun, rows=None):
             raise NotImplementedError("linear: fp32 output with GEGLU or blend")
         if act == 0 and rv is None and a["residual"] is None:
             ref = exact * a["out_scale"] if a["out_scale"] != 1.0 else exact
-            return [_report(name, out, ref, 1e-3, atol * abs(a["out_scale"]), dims=dims)]
+            return [_report(name, out, ref, 1e-3, atol * abs(a["out_scale"]), dims=dims, units=(0,))]
         pre = rerun(**_PRE_ONLY)
         _sync()
-        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims),
+        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims, units=(0,)),
                 _f32_epilogue_verdict(name, pre, out, a, rv, dims)]
     pre = rerun(**_PRE_ONLY)
     _sync()
-    recs = [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims)]
+    recs = [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims, units=(0,))]
     if act == 2:  # GEGLU: value / gate columns interleaved per 256-wide tile (ops.pack_geglu_weight)
         if a["out_scale"] != 1.0 or any(a[k] is not None for k in ("rowvec", "residual", "blend_src")):
             raise NotImplementedError("linear: GEGLU with a further epilogue")
         m, n = pre.shape[0], w.shape[0] // 2
         p4 = pre.to(F64).reshape(m, n // 128, 2, 128)
         h = _r64(torch.cat([p4[:, :, 0].reshape(m, n), p4[:, :, 1].reshape(m, n)], dim=1))
-        recs.append(_report(name, out, _r64(h[:, :n] * _r64(F.gelu(h[:, n:]))), 2 ** -6, 2e-3, dims=dims))
+        recs.append(_report(name, out, _r64(h[:, :n] * _r64(F.gelu(h[:, n:]))), 2 ** -6, 2e-3, dims=dims, units=(0,)))
         return recs
     f64 = (lambda t: None if t is None else t.to(F64))
     ref, rtol, mag = _epilogue_chain64(
         pre.to(F64), act=act, scale=a["out_scale"], res=f64(a["residual"]), xs=f64(a["blend_src"]),
         alpha=a["blend_alpha"], rv=rv)
-    recs.append(_report(name, out, ref, rtol, 1e-3, mag=mag, dims=dims))
+    recs.append(_report(name, out, ref, rtol, 1e-3, mag=mag, dims=dims, units=(0,)))
     return recs
 
 
@@ -789,7 +834,7 @@ def conv2d_verdict(name, a, out, rerun, rows=None):
         rv = a["rowvec"]
         if rv is not None:
             rv = (rv[ii] if rv.shape[0] > 1 else rv).to(F64)[:, None, None, :]
-        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims, rows=rows),
+        return [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, dims=dims, rows=rows, units=(0, 1, 2)),
                 _f32_epilogue_verdict(name, pre, out[ii], {**a, "residual": f64(a["residual"])}, rv, dims, rows)]
     if a["out_fp32"]:
         if a["blend_src"] is not None:
@@ -798,18 +843,18 @@ def conv2d_verdict(name, a, out, rerun, rows=None):
         if a["residual"] is not None:
             ref = ref + f64(a["residual"])
         return [_report(name, out[ii], ref, 1e-3, atol * abs(a["out_scale"]), {"torch_fp32_max_err": fp32_err},
-                        dims=dims, rows=rows)]
+                        dims=dims, rows=rows, units=(0, 1, 2))]
     pre = rerun(**_PRE_ONLY)[ii]
     _sync()
     recs = [_report(f"{name} pre-activation", pre, exact, 1e-3, atol, {"torch_fp32_max_err": fp32_err}, dims=dims,
-                    rows=rows)]
+                    rows=rows, units=(0, 1, 2))]
     del exact
     rv = a["rowvec"]
     if rv is not None:
         rv = (rv[ii] if rv.shape[0] > 1 else rv).to(F64)[:, None, None, :]
     ref, rtol, mag = _epilogue_chain64(pre.to(F64), act=a["act"], scale=a["out_scale"], rv=rv, res=f64(a["residual"]),
                                        xs=f64(a["blend_src"]), alpha=a["blend_alpha"])
-    recs.append(_report(name, out[ii], ref, rtol, 1e-3, mag=mag, dims=dims, rows=rows))
+    recs.append(_report(name, out[ii], ref, rtol, 1e-3, mag=mag, dims=dims, rows=rows, units=(0, 1, 2)))
     return recs
 
 
@@ -837,7 +882,7 @@ def temporal_conv_verdict(name, a, out, frames=None):
     ref, rtol, mag = _epilogue_chain64(acc, rv=rv, res=f64(a["residual"]), xs=f64(a["blend_src"]),
                                        alpha=a["blend_alpha"], multi=True)
     return _report(name, out.reshape(b, f, h * w_, cout)[:, fi], ref, rtol, 1e-3, mag=mag,
-                   dims=("clip", "frame", "pixel", "ch"), rows=None)
+                   dims=("clip", "frame", "pixel", "ch"), rows=None, units=(0, 1, 2))
 
 
 def check_linear_f32_scale(m, n, k, seed=0):
@@ -857,13 +902,18 @@ def _bf16_ulp(a):
 
 
 def _chain_verdict(name, out, ref, tol, extra=None):
-    """out vs a float64 chain at an element-wise tolerance `tol` (the scheduler steps)"""
+    """out vs a float64 chain at an element-wise tolerance `tol` (the scheduler steps), and the direction statistics of
+    tests/error_stats.py over blocks of 4096 elements (elements with |ref| <= tol left out of the bias)"""
     err = (out.to(F64) - ref).abs()
     ratio = torch.where(torch.isfinite(out), err / tol, math.inf)
     bad = int((ratio > 1.0).sum())
     rec = {"max_abs_err": float(err.max()), "max_err_over_tol": float(ratio.max()), "n_bad": bad, "n": out.numel()}
     rec.update(extra or {})
-    return _exact(name, bad == 0 and rec.get("model_in_next_ok", True), rec)
+    del err, ratio
+    stats = es.direction(out, ref, None, tol=tol)
+    rec = _exact(name, bad == 0 and rec.get("model_in_next_ok", True), rec)
+    _add_direction(rec, stats)
+    return rec
 
 
 def _next_input_ok(nxt, out, div):
@@ -1014,7 +1064,8 @@ def latent_encoder_verdict(name, x, clips, frames, params, out):
     y, mag = _latent_encoder_ref64(x, clips, frames, params)
     o4 = out[..., :4].reshape(clips, frames, h * w, 4).permute(0, 2, 1, 3)
     return [_exact(f"{name} channels 4..{x.shape[3] - 1} zero", bool((out[..., 4:] == 0).all())),
-            _report(name, o4, y, 2 ** -6, 1e-3, mag=mag.expand_as(y), dims=("clip", "pixel", "frame", "ch"))]
+            _report(name, o4, y, 2 ** -6, 1e-3, mag=mag.expand_as(y), dims=("clip", "pixel", "frame", "ch"),
+                    units=(0, 1))]
 
 
 def check_latent_encoder(clips, frames, h=10, w=10, c_stride=8, seed=0):
@@ -1044,6 +1095,7 @@ def groupnorm_verdict(name, a, out, samples=None):
     ii = slice(None) if imgs is None else torch.tensor(imgs, device=x.device)
     xin = (x[ii] if x2 is None else torch.cat([x[ii], x2[ii]], dim=3)).to(F64)
     nn, ct = xin.shape[0], xin.shape[3]
+    eager = _groupnorm_eager(xin, a, ips, groups) if xin.numel() <= es.THIN else None  # bounded memory
     t = xin.reshape(nn // ips, ips * h * w, groups, ct // groups)  # in place from here: a 14-frame 576x1024 sample
     t.sub_(t.mean(dim=(1, 3), keepdim=True))                       # is 8.5 GB in float64
     t.mul_(torch.rsqrt(t.square().mean(dim=(1, 3), keepdim=True) + a["eps"]))
@@ -1052,7 +1104,25 @@ def groupnorm_verdict(name, a, out, samples=None):
         y = F.silu(y, inplace=True)
     if a["up2x"]:
         y = y.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-    return _report(name, out[ii], _r64(y), 2 ** -7, 2e-3, dims=("img", "y", "x", "ch"), rows=imgs)
+    # direction: bias over the (sample, group) units, gain per (sample, group) about each channel's beta (SiLU of it),
+    # its se clustered by the (sample, pixel, group) units inside
+    center = a["beta"].to(F64)
+    center = (F.silu(center) if a["silu"] else center).reshape(1, 1, groups, ct // groups)
+    return _report(name, out[ii], _r64(y), 2 ** -7, 2e-3, dims=("img", "y", "x", "ch"), rows=imgs, units=(0, 2),
+                   gain=((0, 2), center, (0, 1, 2)), eager=eager, unit_shape=(nn // ips, -1, groups, ct // groups))
+
+
+def _groupnorm_eager(xin, a, ips, groups):
+    """torch's eager GroupNorm (+ SiLU, + up-sampling) on the same bf16 inputs, fp32 arithmetic, one rounding to bf16:
+    the gain's yardstick"""
+    nn, h, w, ct = xin.shape
+    x3 = xin.float().reshape(nn // ips, ips * h * w, ct).transpose(1, 2)
+    y = F.group_norm(x3, groups, a["gamma"].float(), a["beta"].float(), a["eps"]).transpose(1, 2).reshape(nn, h, w, ct)
+    if a["silu"]:
+        y = F.silu(y)
+    if a["up2x"]:
+        y = y.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
+    return y.to(BF16)
 
 
 def layernorm_verdict(name, a, out):
@@ -1068,7 +1138,10 @@ def layernorm_verdict(name, a, out):
         if ysum is not None:
             recs.append(_report(f"{name} sum", ysum.reshape(-1, c), xf, 0.0, 0.0, dims=("row", "ch")))
     ref = _r64(F.layer_norm(xf, (c,), a["gamma"].to(F64), a["beta"].to(F64), a["eps"]))
-    recs.append(_report(name, y.reshape(-1, c), ref, 2 ** -7, 2e-3, dims=("row", "ch")))
+    # direction: units the rows, gain about beta; yardstick: torch's LayerNorm on the same bf16 input, fp32 arithmetic
+    eager = F.layer_norm(xf.float(), (c,), a["gamma"].float(), a["beta"].float(), a["eps"]).to(BF16)
+    recs.append(_report(name, y.reshape(-1, c), ref, 2 ** -7, 2e-3, dims=("row", "ch"), units=(0,),
+                        gain=((), a["beta"].to(F64), None), eager=eager))
     return recs
 
 

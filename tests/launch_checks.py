@@ -38,6 +38,7 @@ import torch
 import torch.nn.functional as F
 
 from tests import kernel_checks as kc
+from tests.error_stats import BLOCKS as ES_BLOCKS
 
 F64 = torch.float64
 BF16 = torch.bfloat16
@@ -139,11 +140,12 @@ def _v_timestep_embedding(a, out, rerun):
     arg = t[:, None] * freq[None, :]
     ref = torch.cat([torch.cos(arg), torch.sin(arg)] if a["flip_sin_to_cos"] else [torch.sin(arg), torch.cos(arg)], -1)
     ref = F.pad(ref, (0, dim - 2 * half))  # odd dim: a trailing zero column
-    return [kc._report("timestep_embedding", out, kc._r64(ref), 2 ** -7, 4e-3, dims=("t", "ch"))], False
+    return [kc._report("timestep_embedding", out, kc._r64(ref), 2 ** -7, 4e-3, dims=("t", "ch"),
+                       units=ES_BLOCKS)], False
 
 
 def _v_silu(a, out, rerun):
-    return [kc._report("silu", out, kc._r64(F.silu(a["x"].to(F64))), 2 ** -7, 1e-3)], False
+    return [kc._report("silu", out, kc._r64(F.silu(a["x"].to(F64))), 2 ** -7, 1e-3, units=ES_BLOCKS)], False
 
 
 def _v_add(a, out, rerun):
@@ -165,7 +167,8 @@ def _v_nhwc_to_nchw(a, out, rerun):
 
 def _v_avgpool(a, out, rerun):
     ref = F.adaptive_avg_pool2d(a["x"].to(F64).permute(0, 3, 1, 2), (a["oh"], a["ow"])).permute(0, 2, 3, 1)
-    return [kc._report("avgpool", out, kc._r64(ref), 2 ** -7, 1e-3, dims=("img", "y", "x", "ch"))], False
+    return [kc._report("avgpool", out, kc._r64(ref), 2 ** -7, 1e-3, dims=("img", "y", "x", "ch"),
+                       units=(0, 1, 2))], False
 
 
 def _v_upsample2x(a, out, rerun):
@@ -175,7 +178,7 @@ def _v_upsample2x(a, out, rerun):
 
 def _v_softmax_rows(a, out, rerun):
     return [kc._report("softmax_rows", out, torch.softmax(a["x"].to(F64), dim=-1), 2 ** -8, 1e-6,
-                       dims=("row", "col"))], False
+                       dims=("row", "col"), units=(0,))], False
 
 
 def _v_frame_conv_small(a, out, rerun):
@@ -186,14 +189,16 @@ def _v_frame_conv_small(a, out, rerun):
     ref = F.conv3d(xs, a["w_host"].to(x.device, F64)[:, :, :, None, None],
                    None if b is None else b.to(x.device, F64), padding=(1, 0, 0))
     ref = ref.permute(0, 2, 1, 3, 4).reshape(bf, -1, h, w)
-    return [kc._report("frame_conv_small", out, kc._r64(ref), 2 ** -7, 2e-3, dims=("img", "ch", "y", "x"))], False
+    return [kc._report("frame_conv_small", out, kc._r64(ref), 2 ** -7, 2e-3, dims=("img", "ch", "y", "x"),
+                       units=(0, 2, 3))], False
 
 
 def _v_router_weights(a, out, rerun):
     lg = a["logits"].to(F64)
     if a["mask"] is not None:
         lg = torch.where(a["mask"].bool()[None, :], lg, lg - 1e6)
-    return [kc._report("router_weights", out, torch.softmax(lg, dim=-1), 1e-5, 1e-7, dims=("row", "expert"))], False
+    return [kc._report("router_weights", out, torch.softmax(lg, dim=-1), 1e-5, 1e-7, dims=("row", "expert"),
+                       units=(0,))], False
 
 
 def _v_router_merge(a, out, rerun):
@@ -201,7 +206,7 @@ def _v_router_merge(a, out, rerun):
     for x, wk in zip(a["xs"], a["w"].to(F64)):
         term = kc._r64(x.to(F64) * kc._r64(wk))
         acc = term if acc is None else kc._r64(acc + term)
-    return [kc._report("router_merge", out, acc, 0.0, 0.0)], False
+    return [kc._report("router_merge", out, acc, 0.0, 0.0, units=ES_BLOCKS)], False
 
 
 def _v_cfg_euler(a, out, rerun):
@@ -448,6 +453,12 @@ class Row:
             for k in ("torch_fp32_max_err", "sdpa_bf16_max_err"):  # the error of torch's own kernel, for scale
                 if k in r:
                     self.notes[k] = max(self.notes.get(k, 0.0), r[k])
+            if "bias_ulp" in r:  # the direction statistics (tests/error_stats.py): worst statistic over its bound
+                for k, v in (("bias/bound", max(abs(r["bias_ulp"]) / r["bias_bound"],
+                                                abs(r["bias0_ulp"]) / r["bias0_bound"])),
+                             ("gain/bound", r["gain_over_bound"]), ("rms/eager", r.get("rms_ratio", 0.0))):
+                    if v > 0.0:
+                        self.notes[k] = max(self.notes.get(k, 0.0), v)
             ratio = max(r.get("max_err_over_tol", 0.0), r.get("max_bh_err_over_2x_sdpa", 0.0))
             if not r["ok"]:
                 self.fail(f"{r['check']}: {r.get('why') or 'out of tolerance'}")
