@@ -44,6 +44,39 @@ def pool_controlnet_input(latents: torch.Tensor) -> torch.Tensor:
     return as_nchw(ops.avgpool(to_channels_last_bf16(latents, 8), 64, 64))[:, :4]
 
 
+def check_geometry(loop: str, h: int, w: int, use_size_512: bool, control_images, *, multiple: int,
+                   adapter_up: int) -> None:
+    """Refuse, before any kernel runs, latents (h, w) or control images the loop body cannot carry through.
+
+    The ControlNet runs at 64x64 latents when use_size_512 pools a latent size other than 64x64 (the reference's
+    F.adaptive_avg_pool2d, here only at integer ratios), and at the latent size otherwise; its conditioning images are
+    then 512x512 (pooled from integer multiples of 512) or 8 x the ControlNet's latent size.  The adapter returns its
+    residuals at `adapter_up` x the ControlNet's size, and the UNet adds them to skips at the latent size, so the two
+    must agree.  `multiple`: what the latent height and width must be multiples of (the UNet's down-samplers, the
+    ControlNet's stride-2 convolutions when it runs at the latent size, I2VGen-XL's 32x32 image-latent pool).
+    Domain of the three loops: SDXL (2x adapter) runs 128x128 latents with use_size_512; I2VGen-XL runs 64x64 with
+    use_size_512, multiples of 32 without; SVD runs 64x64 with use_size_512, multiples of 8 without."""
+    size = f"latents {h}x{w} (height {8 * h}, width {8 * w})"
+    if h <= 0 or w <= 0 or h % multiple or w % multiple:
+        raise ValueError(f"{loop}: height and width must be multiples of {8 * multiple} pixels (latent height and "
+                         f"width multiples of {multiple}), got {size}")
+    pool = use_size_512 and (h, w) != (64, 64)
+    ch, cw = (64, 64) if pool else (h, w)
+    if (ch * adapter_up, cw * adapter_up) != (h, w):
+        why = "use_size_512 pools the ControlNet input to 64x64" if pool else "the ControlNet runs at the latent size"
+        raise ValueError(f"{loop}: {size} with use_size_512={use_size_512} cannot be run: {why}, the adapter returns "
+                         f"residuals at {ch * adapter_up}x{cw * adapter_up} and the UNet adds them at height x width "
+                         f"{h}x{w}")
+    for img in control_images if isinstance(control_images, (list, tuple)) else [control_images]:
+        ih, iw = img.shape[-2:]
+        if pool and (ih % 512 or iw % 512):
+            raise ValueError(f"{loop}: control images of height {ih} and width {iw}: use_size_512 pools them to "
+                             f"512x512, so height and width must be multiples of 512")
+        if not pool and (ih, iw) != (8 * ch, 8 * cw):
+            raise ValueError(f"{loop}: control images of height {ih} and width {iw}, expected height {8 * ch} and "
+                             f"width {8 * cw} for {size}")
+
+
 class DenoiseLoopBase:
     num_inference_steps: int
 

@@ -294,7 +294,9 @@ def conv2d(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.Tensor]
         os_ = (cout, wo * cout, ho * wo * cout, 0)
         rvs = (0, 0, rowvec.stride(0) if (rowvec is not None and rowvec.shape[0] > 1) else 0, 0)
     else:
-        assert ksize == 3 and x2 is None and h % 2 == 0 and w_ % 2 == 0
+        if ksize != 3 or x2 is not None or h % 2 or w_ % 2:
+            raise ValueError(f"conv2d: stride 2 takes one source, a 3x3 kernel and an even height and width, got "
+                             f"ksize {ksize}, {2 if x2 is not None else 1} sources, height {h}, width {w_}")
         # parity view: channel axis [x parity][C], row dims (x/2, y parity, y/2, n)
         d.a_channels[0] = 2 * c
         d.a_dims[0], d.a_dims[1], d.a_dims[2], d.a_dims[3] = w_ // 2, 2, h // 2, n

@@ -15,7 +15,7 @@ import torch
 
 from . import ops
 from .layers import as_nchw, cache_static_context, to_channels_last_bf16
-from .loop_base import DenoiseLoopBase
+from .loop_base import DenoiseLoopBase, check_geometry
 from .schedulers import DDIMSchedule
 
 BF16 = torch.bfloat16
@@ -48,6 +48,11 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
         """latents (B,4,F,h,w) unit noise; prompt_embeds (2B,77,1024) negative first; image_latents (2B,4,F,h,w);
         image_embeddings (2B,1,1024); fps (2B,); controlnet_prompt_embeds (2B*F,77,768); control_images: (2B*F,3,H,W)
         or a list of E such tensors (Multi-ControlNet)."""
+        # use_size_512: the reference pools the ControlNet input to 64x64, but its video adapters do not up-sample, so
+        # only 64x64 latents (512x512 video) fit the UNet (elsewhere it fails inside the UNet, :689); without it the
+        # image latents' 32x32 pool needs multiples of 32
+        check_geometry("I2VGen-XL loop", *latents.shape[-2:], self.use_size_512, control_images, multiple=32,
+                       adapter_up=1)
         dev = latents.device
         b, c, f, h, w = latents.shape
         self.batch, self.frames = b, f
@@ -63,11 +68,6 @@ class I2VGenXLControlNetAdapterLoop(DenoiseLoopBase):
         self.image_embeddings = image_embeddings.to(BF16).contiguous()
         self.fps = fps.float().contiguous()
         self.cn_embeds = controlnet_prompt_embeds.to(BF16).contiguous()
-        if (h, w) != (64, 64) and self.use_size_512:                                        # :941-947
-            # the reference pools the ControlNet input to 64x64 here, but its video adapters do not up-sample, so the
-            # 64x64 residuals cannot be added to a UNet running at another size (it fails inside the UNet, :689)
-            raise ValueError("use_size_512=True needs 64x64 latents (512x512 video) for the I2VGen-XL backbone; pass "
-                             "use_size_512=False to run the ControlNet at the latent resolution")
         self.images = ([i.to(BF16).contiguous() for i in control_images] if isinstance(control_images, (list, tuple))
                        else control_images.to(BF16).contiguous())
         # adapter context: the LAST sample's image embedding for every sample (reference :1048, quirk Q5)

@@ -15,7 +15,7 @@ import torch
 
 from . import ops
 from .layers import cache_static_context
-from .loop_base import DenoiseLoopBase, pool_control_images, pool_controlnet_input
+from .loop_base import DenoiseLoopBase, check_geometry, pool_control_images, pool_controlnet_input
 from .schedulers import EulerDiscreteSchedule
 
 BF16 = torch.bfloat16
@@ -39,6 +39,8 @@ class SDXLControlNetAdapterLoop(DenoiseLoopBase):
         """latents [B,4,h,w] (unit-variance noise, scaled here by init_noise_sigma as prepare_latents does);
         prompt_embeds [2B,77,2048] (negative first), add_text_embeds [2B,1280], add_time_ids [2B,6],
         controlnet_prompt_embeds [2B,77,768], control_images [2B,3,H,W] in [0,1]."""
+        # the SDXL adapter up-samples 2x: its residuals fit the UNet at 128x128 latents only
+        check_geometry("SDXL loop", *latents.shape[-2:], self.use_size_512, control_images, multiple=4, adapter_up=2)
         dev = latents.device
         self.batch = latents.shape[0]
         self.latents = (latents.float() * self.schedule.init_noise_sigma).to(BF16).float().contiguous()

@@ -18,7 +18,7 @@ import torch
 
 from . import ops
 from .layers import cache_static_context
-from .loop_base import DenoiseLoopBase, pool_control_images, pool_controlnet_input
+from .loop_base import DenoiseLoopBase, check_geometry, pool_control_images, pool_controlnet_input
 from .schedulers import EulerKarrasVSchedule
 
 BF16 = torch.bfloat16
@@ -43,6 +43,7 @@ class SVDControlNetAdapterLoop(DenoiseLoopBase):
         """latents (B,F,4,h,w) unit noise; image_latents (2B,F,4,h,w), zeros for the unconditional half (:225-230,
         :582); image_embeddings (2B,1,1024) negative first; added_time_ids (2B,3); controlnet_prompt_embeds
         (2B*F,77,768); control_images (2B*F,3,H,W) in [0,1]."""
+        check_geometry("SVD loop", *latents.shape[-2:], self.use_size_512, control_images, multiple=8, adapter_up=1)
         dev = latents.device
         b, f = latents.shape[:2]
         self.batch, self.frames = b, f

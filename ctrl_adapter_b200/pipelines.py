@@ -336,6 +336,22 @@ def svd_image_latents(vae, image: torch.Tensor, num_frames: int, num_videos_per_
     return x.unsqueeze(1).repeat(1, num_frames, 1, 1, 1).to(BF16)
 
 
+def sdxl_add_time_ids(batch, height, width, original_size=None, crops_coords_top_left=(0, 0), target_size=None,
+                      negative_original_size=None, negative_crops_coords_top_left=(0, 0), negative_target_size=None):
+    """SDXL micro-conditioning (sdxl pipeline :1185-1219): [2 * batch, 6] fp32 rows original_size +
+    crops_coords_top_left + target_size, negative rows first.  Sizes are (height, width); both default to the
+    generated image's."""
+    original_size = original_size or (height, width)
+    target_size = target_size or (height, width)
+    ids = torch.tensor([list(original_size) + list(crops_coords_top_left) + list(target_size)], dtype=torch.float32)
+    if negative_original_size is not None and negative_target_size is not None:
+        nids = torch.tensor([list(negative_original_size) + list(negative_crops_coords_top_left) +
+                             list(negative_target_size)], dtype=torch.float32)
+    else:
+        nids = ids
+    return torch.cat([nids.repeat(batch, 1), ids.repeat(batch, 1)])
+
+
 # ------------------------------------------------------------------------------------------------------------------
 class SDXLControlNetAdapterPipeline(DiffusionPipeline):
     """sdxl/pipelines/sdxl_controlnet_adapter_pipeline.py:235-275 (constructor), :829-1434 (__call__)."""
@@ -390,8 +406,6 @@ class SDXLControlNetAdapterPipeline(DiffusionPipeline):
             raise NotImplementedError("guidance_rescale / guess_mode / skip_* are unused by the SDXL scripts")
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
-        original_size = original_size or (height, width)
-        target_size = target_size or (height, width)
         device = self._execution_device
         # 3. prompt encodings (:1103-1143)
         if prompt_embeds is None:
@@ -411,14 +425,9 @@ class SDXLControlNetAdapterPipeline(DiffusionPipeline):
         shape = (batch * num_images_per_prompt, 4, height // self.vae_scale_factor, width // self.vae_scale_factor)
         # (user latents are scaled by init_noise_sigma as well, like the reference's prepare_latents)
         lat = latents.to(device).float() if latents is not None else _randn(shape, generator, device)
-        # 7. micro-conditioning (:1185-1219)
-        ids = torch.tensor([list(original_size) + list(crops_coords_top_left) + list(target_size)], dtype=torch.float32)
-        if negative_original_size is not None and negative_target_size is not None:
-            nids = torch.tensor([list(negative_original_size) + list(negative_crops_coords_top_left) +
-                                 list(negative_target_size)], dtype=torch.float32)
-        else:
-            nids = ids
-        add_time_ids = torch.cat([nids.repeat(batch, 1), ids.repeat(batch, 1)]).to(device)
+        add_time_ids = sdxl_add_time_ids(batch, height, width, original_size, crops_coords_top_left, target_size,
+                                         negative_original_size, negative_crops_coords_top_left,
+                                         negative_target_size).to(device)
         loop = SDXLControlNetAdapterLoop(
             self.controlnet, self.adapter, self.unet, num_inference_steps=num_inference_steps,
             guidance_scale=guidance_scale, controlnet_conditioning_scale=_first(controlnet_conditioning_scale),

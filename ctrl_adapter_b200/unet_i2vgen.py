@@ -233,11 +233,7 @@ class I2VGenXLUNet(PretrainedMixin, nn.Module):
         fps_t = fps.to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
         fe = self.fps_embedding[2](self.fps_embedding[0](ops.timestep_embedding(fps_t, 320), act=ACT_SILU))  # [b,1280]
         # context tokens: text (77) + image-latent tokens (64) + image-embedding tokens (4)
-        il_first = image_latents[:, :, 0].contiguous()                        # (b,4,h,w) first frame
-        e = self.image_latents_context_embedding[0](to_channels_last_bf16(il_first, 8), act=ACT_SILU)
-        e = ops.avgpool(e, 32, 32) if (h, w) != (32, 32) else e               # AdaptiveAvgPool2d((32, 32))
-        e = self.image_latents_context_embedding[3](e, act=ACT_SILU)
-        e = self.image_latents_context_embedding[5](e)                        # [b, 8, 8, 1024]
+        e = self.image_latent_tokens(image_latents[:, :, 0].contiguous())      # first frame (b,4,h,w) -> [b,8,8,1024]
         ie = image_embeddings.to(BF16).reshape(-1, image_embeddings.shape[-1]).contiguous()
         ie = self.context_embedding[2](self.context_embedding[0](ie, act=ACT_SILU))
         ie = ie.reshape(-1, self.config.in_channels, self.config.cross_attention_dim)
@@ -249,6 +245,14 @@ class I2VGenXLUNet(PretrainedMixin, nn.Module):
         x = self.image_latents_proj_in[4](x)                                  # [b*f, h, w, 8] (4 real channels)
         il_enc = self.image_latents_temporal_encoder(x, b, f)
         return dict(fps_emb=fe, ctx=ctx, il_enc=il_enc, frames=f)
+
+    def image_latent_tokens(self, il_first):
+        """The first frame's image latents (b, 4, h, w) -> conv -> 32x32 pool -> two stride-2 convs: [b, 8, 8, 1024]
+        channels-last, 64 context tokens per clip (unet_i2vgen_xl.py:210-218, :624)."""
+        e = self.image_latents_context_embedding[0](to_channels_last_bf16(il_first, 8), act=ACT_SILU)
+        e = ops.avgpool(e, 32, 32) if tuple(e.shape[1:3]) != (32, 32) else e  # AdaptiveAvgPool2d((32, 32))
+        e = self.image_latents_context_embedding[3](e, act=ACT_SILU)
+        return self.image_latents_context_embedding[5](e)
 
     def _conditioning(self, fps, image_latents, image_embeddings, encoder_hidden_states):
         key = tuple((t.data_ptr(), t._version, tuple(t.shape)) for t in (fps, image_latents, image_embeddings,

@@ -247,7 +247,7 @@ def test_emulated_i2vgen_loop_multi_controlnet_router():
     from oracle.pipeline_i2vgen import DDIMScheduler, i2vgen_step
     from oracle.unet_i2vgen import I2VGenXLUNet as OU
     from oracle.weights import seeded_tensor
-    b, f, r = 1, 4, 16
+    b, f, r = 1, 4, 32  # the 32x32 image-latent pool needs latents that are multiples of 32
     n = 2 * b * f
     kw = dict(cases.ADAPTER_VIDEO_KW, num_frames=f)
     oad, ad = _pair(lambda: OA(**kw), lambda: ControlNetAdapter(**kw), 2)
@@ -295,7 +295,7 @@ def test_emulated_i2vgen_loop(sparse):
     from oracle.pipeline_i2vgen import DDIMScheduler, i2vgen_step
     from oracle.unet_i2vgen import I2VGenXLUNet as OU
     from oracle.weights import seeded_tensor
-    b, f, r = 1, 4, 16
+    b, f, r = 1, 4, 32  # the 32x32 image-latent pool needs latents that are multiples of 32
     n = 2 * b * f
     kw = dict(cases.ADAPTER_VIDEO_KW, num_frames=f)
     oad, ad = _pair(lambda: OA(**kw), lambda: ControlNetAdapter(**kw), 2)
