@@ -163,6 +163,15 @@ __device__ __forceinline__ void named_bar_arrive(int id, int count) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// stmatrix.m8n8.x4 (b16): stores four 8x8 matrices.  Lane l holds row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1 of
+// matrix i in register ri -- the layout of an mma / wgmma accumulator fragment -- and gives the shared-memory address
+// of row l % 8 of matrix l / 8 (16 bytes, 16-byte aligned).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>

@@ -23,9 +23,10 @@
 //                             both operands read from the 128B-swizzled ring, accumulates in registers, and releases
 //                             a ring slot as soon as the wgmma that read it have retired.  After the last k-iteration
 //                             they wait on `drained` (the storers have finished the previous tile), add the bias
-//                             (copied to shared memory once per tile), round, apply SiLU or GEGLU and the output
-//                             scale with their roundings, write bf16 into the staging tile, arrive on `staged` and
-//                             go straight on to the next tile's main loop.  Consumers issue no global stores.
+//                             (copied to shared memory one tile ahead where two bias buffers fit), round, apply SiLU
+//                             or GEGLU and the output scale with their roundings, write bf16 into the staging tile
+//                             with stmatrix, arrive on `staged` and go straight on to the next tile's main loop.
+//                             Consumers issue no global stores.
 // Every rounding is a bf16 rounding of the reference's autocast chain; the order of the steps is that chain's.
 // fp32 outputs (VAE attention scores, kernel checks) are a separate instantiation without staging: the consumers write
 // them straight from the accumulator registers.
@@ -51,15 +52,14 @@ struct GemmCfg {
   static constexpr uint32_t kBBytes = BN * kBK * 2;   // a multiple of the 1 KB swizzle atom for every BN used
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   // bf16 epilogues stage the tile as kBM rows of kOutCols bf16 in 16-byte chunks.  Rows of a multiple of 8 chunks
-  // are XOR-swizzled (chunk ^ (row & 7)), other rows are padded by one chunk: either way a consumer store (8 rows x
-  // 4 words per warp) and a storer read (8 chunks of one row per quarter warp) hit 32 distinct banks.
+  // are XOR-swizzled (chunk ^ (row & 7)), other rows are padded by one chunk: either way a consumer stmatrix (one
+  // chunk of 8 rows per matrix) and a storer read (8 chunks of one row per quarter warp) hit 32 distinct banks.
   static constexpr bool kStaged = EPI != kEpiF32;
   static constexpr int kOutCols = EPI == kEpiGeglu ? BN / 2 : BN;
   static constexpr int kChunks = kOutCols / 8;
   static constexpr bool kSwizzle = kChunks % 8 == 0;
   static constexpr uint32_t kPitch = kOutCols * 2 + (kSwizzle ? 0 : 16);
   static constexpr uint32_t kStagingBytes = kStaged ? kBM * kPitch : 0;
-  static constexpr uint32_t kBiasBytes = kStaged ? BN * 4 : 0;
   // kOps (bf16 epilogue with a residual and / or blend source, aligned path): a ring of kOpSlabs 8 KB slabs, each
   // [kBM rows][32 columns] of one source, which TMA fills ahead of the storers.  BN 256 and 64 take 2 slabs, which
   // fit beside their ring stages; BN 160 and 128 give up one ring stage either way and then have room for 4.
@@ -68,9 +68,16 @@ struct GemmCfg {
   static constexpr uint32_t kOpBytes = kOpSlabs * kOpSlabBytes;
   // 227 KB per block on H100, minus alignment slack, barriers, staging tile, bias and operand slabs: BN 256 keeps 3
   // ring stages (4 for GEGLU, whose staging tile is half as wide)
+  static constexpr uint32_t kBudget1 = 232448 - 1024 - 256 - kStagingBytes - kOpBytes - (kStaged ? BN * 4 : 0);
+  static constexpr int kStages1 = kBudget1 / kStageBytes > 8 ? 8 : kBudget1 / kStageBytes;
+  // The bias row is double-buffered (the next tile's is written while this one's is read, see the consumers) where
+  // the second buffer costs no ring stage: everywhere but BN 256 GEGLU and BN 256 kOps, which have 768 B to spare.
+  static constexpr int kBiasBufs = !kStaged ? 0 : (kBudget1 - BN * 4) / kStageBytes >= kStages1 ? 2 : 1;
+  static constexpr uint32_t kBiasBytes = kBiasBufs * BN * 4;
   static constexpr uint32_t kBudget = 232448 - 1024 - 256 - kStagingBytes - kBiasBytes - kOpBytes;
   static constexpr int kStagesRaw = kBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  static_assert(kStages == kStages1, "the second bias buffer must not cost a ring stage");
   static constexpr uint32_t kSmemBytes =
       kStages * kStageBytes + kStagingBytes + kBiasBytes + kOpBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(EPI == kEpiBf16 || !kOps, "operand slabs are for the plain bf16 epilogue");
@@ -146,29 +153,19 @@ __device__ __forceinline__ void st8_bf16(__nv_bfloat16* g, uint4 v) {
   }
 }
 
-// the storer's part of the chain on one bf16 pair: row vector, residual, AlphaBlender, each rounded to bf16
+// the storer's part of the chain on one bf16 pair: row vector, residual, AlphaBlender, each rounded to bf16.  The adds
+// are packed bf16 adds, bf16(a + b) with one rounding: the bits of an fp32 add of the two bf16 values rounded to bf16,
+// since that fp32 add is exact unless the exponents differ by more than 15, and then both round to the larger one.
 __device__ __forceinline__ uint32_t gemm_finish_word(uint32_t v, bool rv_on, uint32_t rv, bool res_on, uint32_t rs,
                                                      bool blend_on, uint32_t bs, float alpha_s, float alpha_t) {
-  float v0 = bf16lo_to_float(v), v1 = bf16hi_to_float(v);
-  if (rv_on) {
-    v0 += bf16lo_to_float(rv);
-    v1 += bf16hi_to_float(rv);
-    round2_bf16(v0, v1);
-  }
-  if (res_on) {
-    v0 += bf16lo_to_float(rs);
-    v1 += bf16hi_to_float(rs);
-    round2_bf16(v0, v1);
-  }
+  if (rv_on) v = add_bf16x2(v, rv);
+  if (res_on) v = add_bf16x2(v, rs);
   if (blend_on) {
-    float s0 = alpha_s * bf16lo_to_float(bs), s1 = alpha_s * bf16hi_to_float(bs);
-    float t0 = alpha_t * v0, t1 = alpha_t * v1;
-    round2_bf16(s0, s1);
-    round2_bf16(t0, t1);
-    v0 = s0 + t0;
-    v1 = s1 + t1;
+    const uint32_t s = pack_bf16x2(alpha_s * bf16lo_to_float(bs), alpha_s * bf16hi_to_float(bs));
+    const uint32_t t = pack_bf16x2(alpha_t * bf16lo_to_float(v), alpha_t * bf16hi_to_float(v));
+    v = add_bf16x2(s, t);
   }
-  return pack_bf16x2(v0, v1);
+  return v;
 }
 
 // Storers: write one staged tile.  Thread s takes chunks s, s + 96, ... (row-major over 16-byte chunks, so a warp
@@ -183,6 +180,7 @@ __device__ __forceinline__ void gemm_drain_tile(const GemmParams& p, const uint8
   const bool blend_on = kVec ? kBlend : p.blend_src != nullptr;
   __nv_bfloat16* out = static_cast<__nv_bfloat16*>(p.out);
   const int col0 = tn * Cfg::kOutCols;
+#pragma unroll 1  // unrolled, the eight variants of the BN 256 kernels spill at the storers' 72 registers
   for (int q = s; q < kBM * Cfg::kChunks; q += kStorerThreads) {
     const int r = q / Cfg::kChunks, c = q % Cfg::kChunks, col = col0 + 8 * c;
     const GemmRow g = gemm_row(p, org, lb, r);
@@ -310,50 +308,95 @@ __device__ __forceinline__ void gemm_epilogue_f32(const GemmParams& p, const flo
 }
 
 // Consumers, bf16 outputs: bias (from shared memory), rounding, activation and output scale of the thread's
-// accumulators into the staging tile.  Adding -0.0 is exact for every value, so a missing bias is a bias of -0.0.
-// Scaling a bf16-valued number by 1.0 and rounding it again is exact as well, so the scale is always applied.
-template <class Cfg, int BN, bool kSilu>
+// accumulators into the staging tile.  Steps that cannot change a bit are left out, chosen per launch:
+//   kBias = false (no bias): adding -0.0 is exact for every value, NaN included (F2FP gives every NaN the one bf16 NaN);
+//   kScale = false (scale 1): x * 1.0 is exact, and rounding to bf16 before the pack, which rounds to nearest even
+//   itself, gives the same bf16, so the last rounding before the pack is left to the pack.
+// With a scale but no bias, bias_s holds -0.0.
+// The accumulator fragment of 8 columns x 8 rows is an stmatrix m8n8 fragment and one row of it is one 16-byte staging
+// chunk, so each stmatrix.x4 stores chunks j and j + 1 of the warp's 16 rows.  chunk_off(r, c + 8) =
+// chunk_off(r, c) + 128 in both pitch forms, so four per-lane row addresses serve every chunk pair.
+template <class Cfg, int BN, bool kSilu, bool kBias, bool kScale>
 __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float (&acc)[BN / 2], const float* bias_s,
-                                                uint8_t* staging, int r0, int lane) {
+                                                uint8_t* staging, int wrow, int lane) {
   const int q = lane & 3;
+  const int row = wrow + (lane & 8) + (lane & 7);  // matrix lane / 8 = (chunk j + lane / 16, rows +8 (lane / 8 % 2))
+  uint32_t addr[4];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = r0 + 8 * h;
-    if constexpr (Cfg::kOutCols == BN) {
+  for (int i = 0; i < 4; ++i) addr[i] = smem_u32(staging) + Cfg::chunk_off(row, 2 * i + (lane >> 4));
+  auto bias2 = [&](int col) {
+    return kBias ? *reinterpret_cast<const float2*>(bias_s + col) : make_float2(-0.0f, -0.0f);
+  };
+  if constexpr (Cfg::kOutCols == BN) {
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const float2 b = *reinterpret_cast<const float2*>(bias_s + 8 * j + 2 * q);
-        float v0 = acc[4 * j + 2 * h] + b.x, v1 = acc[4 * j + 2 * h + 1] + b.y;
-        round2_bf16(v0, v1);
+    for (int j = 0; j < BN / 8; j += 2) {
+      uint32_t w[4];
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const int jj = j + (m >> 1), h = m & 1;
+        const float2 b = bias2(8 * jj + 2 * q);
+        float v0 = acc[4 * jj + 2 * h], v1 = acc[4 * jj + 2 * h + 1];
+        if constexpr (kBias) {
+          v0 += b.x;
+          v1 += b.y;
+        }
+        if constexpr (kSilu || kScale) round2_bf16(v0, v1);
         if constexpr (kSilu) {
           v0 = __fdividef(v0, 1.0f + __expf(-v0));
           v1 = __fdividef(v1, 1.0f + __expf(-v1));
-          round2_bf16(v0, v1);
+          if constexpr (kScale) round2_bf16(v0, v1);
         }
-        v0 *= p.out_scale;
-        v1 *= p.out_scale;
-        *reinterpret_cast<uint32_t*>(staging + Cfg::chunk_off(r, j) + 4 * q) = pack_bf16x2(v0, v1);
+        if constexpr (kScale) {
+          v0 *= p.out_scale;
+          v1 *= p.out_scale;
+        }
+        w[m] = pack_bf16x2(v0, v1);
       }
-    } else {
-      // GEGLU: weight rows of tile tn are [value rows of BN/2 output columns][the matching gate rows]
+      stmatrix_x4(addr[(j & 7) >> 1] + (j >> 3) * 128, w[0], w[1], w[2], w[3]);
+    }
+  } else {
+    // GEGLU: weight rows of tile tn are [value rows of BN/2 output columns][the matching gate rows]
 #pragma unroll
-      for (int j = 0; j < BN / 16; ++j) {
-        const float2 ba = *reinterpret_cast<const float2*>(bias_s + 8 * j + 2 * q);
-        const float2 bg = *reinterpret_cast<const float2*>(bias_s + BN / 2 + 8 * j + 2 * q);
-        float a0 = acc[4 * j + 2 * h] + ba.x, a1 = acc[4 * j + 2 * h + 1] + ba.y;
-        float g0 = acc[4 * (j + BN / 16) + 2 * h] + bg.x, g1 = acc[4 * (j + BN / 16) + 2 * h + 1] + bg.y;
+    for (int j = 0; j < BN / 16; j += 2) {
+      uint32_t w[4];
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const int jj = j + (m >> 1), h = m & 1;
+        const float2 ba = bias2(8 * jj + 2 * q), bg = bias2(BN / 2 + 8 * jj + 2 * q);
+        float a0 = acc[4 * jj + 2 * h], a1 = acc[4 * jj + 2 * h + 1];
+        float g0 = acc[4 * (jj + BN / 16) + 2 * h], g1 = acc[4 * (jj + BN / 16) + 2 * h + 1];
+        if constexpr (kBias) {
+          a0 += ba.x;
+          a1 += ba.y;
+          g0 += bg.x;
+          g1 += bg.y;
+        }
         round2_bf16(a0, a1);
         round2_bf16(g0, g1);
         float l0 = gelu_erf(g0), l1 = gelu_erf(g1);
         round2_bf16(l0, l1);
         float v0 = a0 * l0, v1 = a1 * l1;
-        round2_bf16(v0, v1);
-        v0 *= p.out_scale;
-        v1 *= p.out_scale;
-        *reinterpret_cast<uint32_t*>(staging + Cfg::chunk_off(r, j) + 4 * q) = pack_bf16x2(v0, v1);
+        if constexpr (kScale) {
+          round2_bf16(v0, v1);
+          v0 *= p.out_scale;
+          v1 *= p.out_scale;
+        }
+        w[m] = pack_bf16x2(v0, v1);
       }
+      stmatrix_x4(addr[(j & 7) >> 1] + (j >> 3) * 128, w[0], w[1], w[2], w[3]);
     }
   }
+}
+
+template <class Cfg, int BN, bool kSilu>
+__device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float (&acc)[BN / 2], const float* bias_s,
+                                                uint8_t* staging, int wrow, int lane) {
+  if (p.out_scale != 1.0f)
+    gemm_stage_tile<Cfg, BN, kSilu, true, true>(p, acc, bias_s, staging, wrow, lane);
+  else if (p.bias != nullptr)
+    gemm_stage_tile<Cfg, BN, kSilu, true, false>(p, acc, bias_s, staging, wrow, lane);
+  else
+    gemm_stage_tile<Cfg, BN, kSilu, false, false>(p, acc, bias_s, staging, wrow, lane);
 }
 
 template <int BN, int EPI, bool kOps>
@@ -496,17 +539,27 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
   const int cw = (warp >> 2) - 1;   // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
   const int wq = warp & 3;          // warp inside the warpgroup: rows [16 wq, 16 wq + 16) of those
   const int ct = threadIdx.x - 128; // consumer thread 0..255
-  const int r0 = cw * 64 + wq * 16 + (lane >> 2);  // the thread's accumulator rows are r0 and r0 + 8
+  const int wrow = cw * 64 + wq * 16;             // the warp's 16 rows
+  const int r0 = wrow + (lane >> 2);              // the thread's accumulator rows are r0 and r0 + 8
   float acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0, staged_phase = 0;
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+  // this thread's bias value (column ct of the tile) of tile t
+  auto bias_of = [&](int t) {
+    const int tn = t % p.n_tiles_n;
+    float b = -0.0f;
+    if (Cfg::kStaged && p.bias != nullptr && ct < BN && t < total_tiles && (EPI == kEpiGeglu || tn * BN + ct < p.n_out))
+      b = __ldg(p.bias + tn * BN + ct);
+    return b;
+  };
+  // with two bias buffers the first tile's bias goes to buffer 0 now (made visible by a barrier in its epilogue)
+  if (Cfg::kBiasBufs == 2 && ct < BN) bias_s[ct] = bias_of(blockIdx.x);
+  for (int tile = blockIdx.x, i = 0; tile < total_tiles; tile += gridDim.x, ++i) {
     int tn, org[4];
     tile_coords(tile, tn, org);
-    // this thread's bias value of the tile, loaded now so that its latency hides behind the main loop
-    float bias_v = -0.0f;
-    if (Cfg::kStaged && p.bias != nullptr && ct < BN && (EPI == kEpiGeglu || tn * BN + ct < p.n_out))
-      bias_v = __ldg(p.bias + tn * BN + ct);
+    // the bias value the epilogue writes to shared memory, loaded now so that its latency hides behind the main loop:
+    // the next tile's with two bias buffers, this tile's with one
+    const float bias_v = bias_of(Cfg::kBiasBufs == 2 ? tile + gridDim.x : tile);
     int prev = -1;
     for (int it = 0; it < kiters; ++it) {
       mbar_wait(&full_bar[stage], phase);
@@ -531,13 +584,25 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_const
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
     if constexpr (Cfg::kStaged) {
-      mbar_wait(drained_bar, staged_phase ^ 1);  // the storers are done with the previous tile (and its bias)
-      if (ct < BN) bias_s[ct] = bias_v;
-      named_bar_sync(1, kConsumerThreads);
+      mbar_wait(drained_bar, staged_phase ^ 1);  // the storers are done with the previous tile
+      const float* bias_t = bias_s;
+      if constexpr (Cfg::kBiasBufs == 2) {
+        // Tile i reads buffer i % 2, which every consumer wrote in the epilogue of tile i - 1 before arriving on
+        // `staged`; the storers arrive on `drained` only after `staged` completed, and this thread waited on `drained`
+        // just above, so those writes are visible (mbarrier arrive releases, wait acquires).  The same chain orders
+        // this thread's write of buffer (i + 1) % 2 below after every consumer's reads of it in tile i - 1.  The first
+        // tile's bias was written before the main loop, with no such chain: the consumers sync once.
+        if (i == 0) named_bar_sync(1, kConsumerThreads);
+        if (ct < BN) bias_s[((i + 1) & 1) * BN + ct] = bias_v;
+        bias_t = bias_s + (i & 1) * BN;
+      } else {
+        if (ct < BN) bias_s[ct] = bias_v;
+        named_bar_sync(1, kConsumerThreads);
+      }
       if (EPI == kEpiBf16 && p.act == CA_ACT_SILU)
-        gemm_stage_tile<Cfg, BN, true>(p, acc, bias_s, staging, r0, lane);
+        gemm_stage_tile<Cfg, BN, true>(p, acc, bias_t, staging, wrow, lane);
       else
-        gemm_stage_tile<Cfg, BN, false>(p, acc, bias_s, staging, r0, lane);
+        gemm_stage_tile<Cfg, BN, false>(p, acc, bias_t, staging, wrow, lane);
       mbar_arrive(staged_bar);
       staged_phase ^= 1;
     } else {
