@@ -92,7 +92,9 @@ struct GemmCfg {
 };
 
 // exact-erf GELU of a bf16-valued x (erf of Abramowitz & Stegun 7.1.26, |error| <= 1.5e-7), arranged as
-// relu(x) - |x| * q(|x|) with q = 0.5 * erfc(|x| / sqrt 2): no cancellation for negative x, no branches
+// relu(x) - |x| * q(|x|) with q = 0.5 * erfc(|x| / sqrt 2): no cancellation for negative x, no branches.
+// At x = +inf, q is 0 and |x| * q is NaN, so +inf is passed through (x * Phi(x) = inf); -inf and NaN give NaN as
+// x * Phi(x) does.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float a = fabsf(x);
   float t;
@@ -105,7 +107,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
   const float arg = (a * a) * (-0.5f * 1.4426950408889634f);
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(arg));
   const float q = (p * t) * e;
-  return fmaf(-a, q, fmaxf(x, 0.0f));
+  return x == INFINITY ? x : fmaf(-a, q, fmaxf(x, 0.0f));
 }
 
 // output row r of a tile with origin `org` -> 4-D output point; lb = log2 of the box extents

@@ -37,6 +37,11 @@ def _epilogue(acc, bias, act, out_scale, rowvec, residual, blend_src, blend_alph
     v = _r(v)
     if act == ACT_SILU:
         v = _r(F.silu(v))
+    return _finish(v, out_scale, rowvec, residual, blend_src, blend_alpha)
+
+
+def _finish(v, out_scale, rowvec, residual, blend_src, blend_alpha):
+    """the bf16 chain after the activation: output scale, row vector, residual, AlphaBlender, each rounded"""
     if out_scale != 1.0:
         v = _r(v * out_scale)
     if rowvec is not None:
@@ -53,22 +58,23 @@ def linear(x, w, bias=None, *, act=ACT_NONE, residual=None, rowvec=None, rows_pe
            out_scale=1.0, out=None, out_fp32=False, bn=0):
     m, k = x.shape
     xf, wf = x.float(), w.float()
+    rv = None
+    if rowvec is not None:
+        assert rows_per_vec > 0 and m % rows_per_vec == 0 and rowvec.shape[0] == m // rows_per_vec
+        rv = rowvec.repeat_interleave(rows_per_vec, dim=0)
     if act == ACT_GEGLU:
-        d = w.shape[0] // 2
-        wt = wf.reshape(d // 128, 2, 128, k)
+        # value and gate rows interleaved per N tile of bn (ops.pack_geglu_weight); bn 0 is ca_gemm's GEGLU tile, 256
+        d, half = w.shape[0] // 2, (bn or 256) // 2
+        wt = wf.reshape(d // half, 2, half, k)
         a = xf @ wt[:, 0].reshape(d, k).t()
         g = xf @ wt[:, 1].reshape(d, k).t()
         if bias is not None:
-            bt = bias.float().reshape(d // 128, 2, 128)
+            bt = bias.float().reshape(d // half, 2, half)
             a = a + bt[:, 0].reshape(d)
             g = g + bt[:, 1].reshape(d)
         a, g = _r(a), _r(g)
-        y = _r(a * _r(F.gelu(g))).to(BF16)
+        y = _finish(_r(a * _r(F.gelu(g))), out_scale, rv, residual, blend_src, blend_alpha)
     else:
-        rv = None
-        if rowvec is not None:
-            assert rows_per_vec > 0 and m % rows_per_vec == 0 and rowvec.shape[0] == m // rows_per_vec
-            rv = rowvec.repeat_interleave(rows_per_vec, dim=0)
         y = _epilogue(xf @ wf.t(), bias, act, out_scale, rv, residual, blend_src, blend_alpha, out_fp32)
     if out is not None:
         out.copy_(y)
