@@ -17,10 +17,12 @@ The fp32-output instantiation keeps fp32 throughout, rounding only after the row
 
 accumulators(): the fp32 accumulators of a call -- the same op, operands, geometry and N tile with fp32 output and an
 empty epilogue (no bias, no activation, scale 1, no row vector / residual / blend), which shares the main loop and so
-the summation order of the bf16 instantiations at that N tile.  expected(): the chain above in torch fp32 on the
-accumulators' device.  compare(): bits against bits, with a diagnosis of a mismatch.  Used by
-tests/test_gemm_epilogue_exact_gpu.py on the kernels and by tests/test_gemm_epilogue_exact_cpu.py on
-tests/ops_emulator.py.
+the summation order of the bf16 instantiations at that N tile.  accumulator_verdict(): those accumulators against the
+float64 contraction of the same operands, so that a main-loop error every instantiation shares (a wrong tap, a dropped
+K block) cannot hide in them.  expected(): the chain above in torch fp32 on the accumulators' device.  compare(): bits
+against bits, with a diagnosis of a mismatch.  slot() / guard_intact(): an output view inside a buffer of sentinel
+bits, and whether a call left those bits alone.  Used by tests/test_gemm_epilogue_exact_gpu.py on the kernels and by
+tests/test_gemm_epilogue_exact_cpu.py on tests/ops_emulator.py.
 """
 from __future__ import annotations
 
@@ -28,7 +30,7 @@ import inspect
 
 import torch
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 ACT_NONE, ACT_SILU, ACT_GEGLU = 0, 1, 2
 STEPS = ("bias", "act", "scale", "rowvec", "residual", "blend")
 
@@ -67,20 +69,43 @@ _EMPTY = dict(bias=None, act=ACT_NONE, out_scale=1.0, rowvec=None, residual=None
 
 
 def accumulators(op, call, ops):
-    """-> (acc, gate_acc): the call's fp32 accumulators in its output's shape; for GEGLU the value and gate halves
-    (the packed weight run as a plain GEMM at the same N tile), else gate_acc is None"""
+    """-> the call's fp32 accumulators in its output's shape; for GEGLU those of the packed weight run as a plain GEMM
+    at the same N tile, value and gate columns interleaved per tile (geglu_halves splits them)"""
     if op == "temporal_conv":
-        return _temporal_conv_fp32(call, ops), None
+        return _temporal_conv_fp32(call, ops)
     fn = getattr(ops, op)
     params = inspect.signature(fn).parameters
     kw = dict(call)
     kw.update({k: v for k, v in _EMPTY.items() if k in params})
     if "bn" in params:
         kw["bn"] = resolved_bn(op, call)
-    acc = fn(**kw)
-    if call.get("act", ACT_NONE) == ACT_GEGLU:
-        return geglu_halves(acc, kw["bn"])
-    return acc, None
+    return fn(**kw)
+
+
+def accumulator_verdict(label, op, call, acc, atol_cap=1e-3):
+    """acc (accumulators()) against the float64 contraction of the call's operands, without the bias: the census's
+    pre-activation bound, rtol 1e-3 and atol max(1e-4, 2^-16 sum |x_k w_k|) (kernel_checks._sum_floor), the atol capped
+    at atol_cap; with the direction statistics of kernel_checks._report.  A convolution over more than 4 images is
+    evaluated on the first, middle and last.  -> the record"""
+    from tests import kernel_checks as kc
+    rows = None
+    if op == "linear":
+        x, w = call["x"].to(F64), call["w"].to(F64)
+        exact, abs_sum = x @ w.t(), x.abs() @ w.abs().t()
+        dims, units = ("row", "col"), (0,)
+    elif op == "conv2d":
+        n = call["x"].shape[0]
+        rows = [0, n // 2, n - 1] if n > 4 else None
+        exact, abs_sum = kc.conv2d_ref({**call, "bias": None}, rows)
+        acc = acc if rows is None else acc[rows]
+        dims, units = ("img", "y", "x", "ch"), (0, 1, 2)
+    else:
+        exact, abs_sum = kc.temporal_conv_ref({**call, "bias": None})
+        acc = acc.reshape(exact.shape)
+        dims, units = ("clip", "frame", "pixel", "ch"), (0, 1, 2)
+    atol = kc._sum_floor(abs_sum).clamp_(max=atol_cap)
+    del abs_sum
+    return kc._report(f"{label} accumulators", acc, exact, 1e-3, atol, dims=dims, rows=rows, units=units)
 
 
 def _temporal_conv_fp32(call, ops):
@@ -166,6 +191,30 @@ def present_steps(kw):
 
 def _int_view(t):
     return t.view(torch.int16) if t.dtype == BF16 else t.view(torch.int32)
+
+
+SENTINEL = -1  # the bits around a slot: all ones, a NaN in bf16 and in fp32
+
+
+def slot(t, left=4, right=12, flat=False):
+    """t's values in columns [left, left + n) of a [rows, left + n + right] buffer whose other elements hold SENTINEL;
+    flat=True: in a contiguous view at element `left` of a flat buffer (a convolution's channels-last output).
+    left = 4 bf16 puts the view 8 bytes off 16-byte alignment"""
+    if flat:
+        return slot(t.reshape(1, -1), left, right).view(t.shape)
+    buf = torch.empty(*t.shape[:-1], left + t.shape[-1] + right, device=t.device, dtype=t.dtype)
+    _int_view(buf).fill_(SENTINEL)
+    view = buf[..., left:left + t.shape[-1]]
+    view.copy_(t)
+    return view
+
+
+def guard_intact(view):
+    """every element of the buffer of a slot() view outside the view still holds SENTINEL"""
+    buf = view._base
+    outside = torch.ones(buf.shape, dtype=torch.bool, device=buf.device)
+    outside.as_strided(view.shape, view.stride(), view.storage_offset()).fill_(False)
+    return bool((_int_view(buf)[outside] == SENTINEL).all())
 
 
 def compare(label, out, acc, chain, *, n_tile_cols):

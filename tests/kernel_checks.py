@@ -1,6 +1,8 @@
-"""GPU parity checks of every CUDA kernel against a plain PyTorch fp32 reference of the same op on the same
+"""GPU parity checks of the CUDA kernels against a plain PyTorch fp32 reference of the same op on the same
 bf16-quantised inputs.  Used by tests/test_kernels_gpu.py (pytest -m gpu), by __graft_entry__.smoke() and as a
-stand-alone report:  python -m tests.kernel_checks  [--group gemm|conv|attn|misc|layouts]  [--json out.json]
+stand-alone report:  python -m tests.kernel_checks  [--group attn|misc|layouts]  [--json out.json]
+The GEMM kernel (linears and convolutions) is checked bit for bit by tests/test_gemm_epilogue_exact_gpu.py, its
+accumulators against float64 with conv2d_ref / temporal_conv_ref below; check_linear and check_conv remain for smoke().
 
 The `layouts` group (LAYOUT_CHECKS, run by tests/test_kernel_layouts_gpu.py) calls the kernels the way the pipelines
 do -- Q/K/V as views of one fused projection, shared per-clip contexts, 17..32 frames, every bf16 GEMM epilogue
@@ -34,6 +36,7 @@ import torch
 import torch.nn.functional as F
 
 from tests import error_stats as es
+from tests.abi_domain import gemm_bn
 
 BF16 = torch.bfloat16
 F64 = torch.float64
@@ -127,83 +130,15 @@ def _add_direction(rec, stats):
 # ------------------------------------------------------------------------------------------------
 # linear
 # ------------------------------------------------------------------------------------------------
-def check_linear(m, k, n, *, bn=0, bias=True, out_fp32=True, residual=False, act="none", seed=0):
+def check_linear(m, k, n, seed=0):
+    """fp32-output linear with bias vs torch fp32 at rtol 1e-3 / atol 1e-4 (__graft_entry__.smoke)"""
     ops = _ops()
     x = _rand(m, k, seed=seed + 1)
     w = _rand(n, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
-    b = _rand(n, seed=seed + 3) if bias else None
-    res = _rand(m, n, seed=seed + 4) if residual else None
-    ref = x.float() @ w.float().t()
-    if b is not None:
-        ref = ref + b.float()
-    if not out_fp32:
-        ref = ref.to(BF16).float()
-    if act == "silu":
-        ref = F.silu(ref).to(BF16).float()
-    mag = ref.abs().clone()
-    if residual:
-        ref = (ref + res.float()).to(BF16).float()
-        mag = torch.maximum(mag, res.float().abs())
-    out = ops.linear(x, w, ops.bias_f32(b), act=ops.ACT_SILU if act == "silu" else ops.ACT_NONE, residual=res,
-                     out_fp32=out_fp32, bn=bn)
+    b = ops.bias_f32(_rand(n, seed=seed + 3))
+    out = ops.linear(x, w, b, out_fp32=True)
     _sync()
-    rtol, atol = (1e-3, 1e-4) if out_fp32 else (2 ** -6 if residual else 2 ** -7, 1e-3)
-    return _report(f"linear m{m} k{k} n{n} bn{bn} {'f32' if out_fp32 else 'bf16'} act={act} res={int(residual)}",
-                   out, ref, rtol, atol, mag=mag)
-
-
-def check_geglu(m, k, d, seed=0):
-    ops = _ops()
-    x = _rand(m, k, seed=seed + 1)
-    w = _rand(2 * d, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
-    b = _rand(2 * d, seed=seed + 3)
-    wi, bi = ops.pack_geglu_weight(w, b, 256)
-    out = ops.linear(x, wi, ops.bias_f32(bi), act=ops.ACT_GEGLU, bn=256)
-    # the same contraction (same kernel, tiles and summation order) with the fp32 pre-activation as output
-    pre = ops.linear(x, wi, ops.bias_f32(bi), out_fp32=True, bn=256).reshape(m, d // 128, 2, 128)
-    pre = torch.cat([pre[:, :, 0].reshape(m, d), pre[:, :, 1].reshape(m, d)], dim=1)  # undo the per-tile interleave
-    _sync()
-    # (1) the contraction against the exact (fp64) pre-activation at the fp32 GEMM tolerance of check_linear
-    exact = (x.double() @ w.double().t() + b.double()).float()
-    _report(f"geglu pre-activation m{m} k{k} d{2 * d}", pre, exact, 1e-3, 1e-4)
-    # (2) the epilogue's bf16 rounding chain applied to the pre-activation the kernel accumulated.  A pre-activation
-    # within an fp32 ulp or two of a bf16 rounding tie rounds either way depending on the summation order (cuBLAS's
-    # own fp32 result rounds ~3300 of the 25.6 M pre-activations at m5000 away from the exact value), and GELU times
-    # the value half magnifies that one-ulp flip beyond the output tolerance, so the epilogue is checked against the
-    # input it was given.
-    h = pre.to(BF16).float()
-    a, g = h[:, :d], h[:, d:]
-    ref = (a * F.gelu(g).to(BF16).float()).to(BF16).float()
-    return _report(f"geglu m{m} k{k} d{d}", out, ref, 2 ** -6, 2e-3)
-
-
-def check_linear_rowvec(m, k, n, rpv, seed=0):
-    ops = _ops()
-    x = _rand(m, k, seed=seed + 1)
-    w = _rand(n, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
-    rv = _rand(m // rpv, n, seed=seed + 3)
-    lin = (x.float() @ w.float().t()).to(BF16).float()
-    ref = (lin + rv.float().repeat_interleave(rpv, dim=0)).to(BF16).float()
-    out = ops.linear(x, w, None, rowvec=rv, rows_per_vec=rpv)
-    _sync()
-    return _report(f"linear+rowvec m{m} k{k} n{n} rpv{rpv}", out, ref, 2 ** -6, 1e-3, mag=lin)
-
-
-def check_linear_blend(m, k, n, seed=0):
-    ops = _ops()
-    x = _rand(m, k, seed=seed + 1)
-    w = _rand(n, k, scale=1.0 / math.sqrt(k), seed=seed + 2)
-    res = _rand(m, n, seed=seed + 4)
-    xs = _rand(m, n, seed=seed + 5)
-    alpha = torch.sigmoid(torch.tensor([0.3], device=DEVICE)).to(BF16)
-    lin = (x.float() @ w.float().t()).to(BF16).float()
-    xt = (lin + res.float()).to(BF16)
-    ref = ((alpha * xs).to(BF16) + ((1.0 - alpha).to(BF16) * xt).to(BF16)).float()
-    out = ops.linear(x, w, None, residual=res, blend_src=xs, blend_alpha=alpha.float())
-    _sync()
-    mag = torch.maximum(torch.maximum(xt.float().abs(), res.float().abs()), xs.float().abs())
-    mag = torch.maximum(mag, lin.abs())  # bf16(x @ w^T) is the first rounded intermediate of the epilogue
-    return _report(f"linear+res+blend m{m} k{k} n{n}", out, ref, 2 ** -7, 1e-3, mag=mag)
+    return _report(f"linear m{m} k{k} n{n} f32", out, x.float() @ w.float().t() + b, 1e-3, 1e-4)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -213,54 +148,16 @@ def _nhwc(x_nchw):
     return x_nchw.permute(0, 2, 3, 1).contiguous()
 
 
-def check_conv(n, h, w, cin, cout, *, ksize=3, stride=1, cin2=0, out_fp32=True, rowvec=False, residual=False,
-               scale=1.0, seed=0):
+def check_conv(n, h, w, cin, cout, seed=0):
+    """fp32-output 3x3 conv with bias vs torch fp32 at rtol 1e-3 / atol 1e-4 (__graft_entry__.smoke)"""
     ops = _ops()
     x = _rand(n, cin, h, w, seed=seed + 1)
-    x2 = _rand(n, cin2, h, w, seed=seed + 5) if cin2 else None
-    ct = cin + cin2
-    wt = _rand(cout, ct, ksize, ksize, scale=1.0 / math.sqrt(ct * ksize * ksize), seed=seed + 2)
-    b = _rand(cout, seed=seed + 3)
-    xin = x.float() if x2 is None else torch.cat([x.float(), x2.float()], dim=1)
-    ref = F.conv2d(xin, wt.float(), b.float(), stride=stride, padding=(ksize - 1) // 2)
-    if not out_fp32:
-        ref = ref.to(BF16).float()
-    if scale != 1.0:
-        ref = (ref * scale).to(BF16).float()
-    rv = res = None
-    mag = ref.abs().clone()
-    if rowvec:
-        rv = _rand(n, cout, seed=seed + 6)
-        ref = (ref + rv.float()[:, :, None, None]).to(BF16).float()
-        mag = torch.maximum(mag, ref.abs())
-    if residual:
-        res = _rand(n, cout, ref.shape[2], ref.shape[3], seed=seed + 7)
-        ref = (ref + res.float()).to(BF16).float()
-        mag = torch.maximum(mag, res.float().abs())
-    kpad = 64 if stride == 2 else 8
-    wp = ops.pack_conv_weight(wt, kpad)
-    out = ops.conv2d(_nhwc(x), wp, ops.bias_f32(b), ksize=ksize, stride=stride, x2=_nhwc(x2) if x2 is not None else None,
-                     out_fp32=out_fp32, rowvec=rv, residual=_nhwc(res) if res is not None else None, out_scale=scale)
+    wt = _rand(cout, cin, 3, 3, scale=1.0 / math.sqrt(cin * 9), seed=seed + 2)
+    b = ops.bias_f32(_rand(cout, seed=seed + 3))
+    ref = F.conv2d(x.float(), wt.float(), b, padding=1)
+    out = ops.conv2d(_nhwc(x), ops.pack_conv_weight(wt), b, out_fp32=True)
     _sync()
-    rtol, atol = (1e-3, 1e-4) if out_fp32 else (2 ** -6 if (rowvec or residual) else 2 ** -7, 1e-3)
-    return _report(f"conv{ksize}x{ksize} s{stride} n{n} {h}x{w} c{cin}+{cin2}->{cout} {'f32' if out_fp32 else 'bf16'}"
-                   f" rv={int(rowvec)} res={int(residual)} sc={scale}", out.permute(0, 3, 1, 2), ref, rtol, atol, mag=mag)
-
-
-def check_temporal_conv(b, f, h, w, c, cout, seed=0):
-    ops = _ops()
-    x = _rand(b, c, f, h, w, seed=seed + 1)
-    wt = _rand(cout, c, 3, 1, 1, scale=1.0 / math.sqrt(3 * c), seed=seed + 2)
-    bias = _rand(cout, seed=seed + 3)
-    rv = _rand(b * f, cout, seed=seed + 4)
-    ref = F.conv3d(x.float(), wt.float(), bias.float(), padding=(1, 0, 0)).to(BF16).float()
-    mag = ref.abs().clone()
-    ref = (ref + rv.float().reshape(b, f, cout).permute(0, 2, 1)[:, :, :, None, None]).to(BF16).float()
-    xl = x.permute(0, 2, 3, 4, 1).reshape(b * f, h, w, c).contiguous()
-    out = ops.temporal_conv(xl, ops.pack_conv_weight(wt), ops.bias_f32(bias), f, rowvec=rv)
-    _sync()
-    out5 = out.reshape(b, f, h, w, cout).permute(0, 4, 1, 2, 3)
-    return _report(f"temporal_conv b{b} f{f} {h}x{w} c{c}->{cout}", out5, ref, 2 ** -6, 1e-3, mag=mag)
+    return _report(f"conv3x3 n{n} {h}x{w} c{cin}->{cout} f32", out.permute(0, 3, 1, 2), ref, 1e-3, 1e-4)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -487,17 +384,6 @@ def _exact(name, ok, extra=None):
     return rec
 
 
-def _default_bn(w_rows, geglu=False):
-    """the tile width ca_gemm picks when bn = 0"""
-    if geglu or w_rows % 256 == 0:
-        return 256
-    if w_rows % 160 == 0:
-        return 160
-    if w_rows % 128 == 0:
-        return 128
-    return 64 if w_rows <= 64 else 128 if w_rows <= 128 else 256
-
-
 def _attn_ref64(q, k, v, kv_idx, scale, chunk=256):
     """q [B, Lq, H, d], k / v [Bk, Lk, H, d]; query batch b attends to K/V batch kv_idx[b].  float64, query axis in chunks
     so that the score matrix stays small."""
@@ -650,7 +536,7 @@ def check_gemm_epilogue(kind, m, k, n, rows_per_vec=0, seed=0):
     obuf = torch.full((m, n + 16), 7.0, device=DEVICE, dtype=BF16)
     ops.linear(x, wk, bias, rowvec=slot(rv), residual=slot(res), blend_src=slot(xs), out=obuf[:, 4:4 + n], **kw)
     _sync()
-    name = f"gemm epilogue {kind} m{m} k{k} n{n} bn{_default_bn(w_rows, geglu)}"
+    name = f"gemm epilogue {kind} m{m} k{k} n{n} bn{gemm_bn(w_rows, geglu)}"
     linear_verdict(name, call, out, lambda **changes: ops.linear(**{**call, **changes}))
     same = torch.equal(obuf[:, 4:4 + n].view(torch.int16), out.view(torch.int16))
     n_diff = int((obuf[:, 4:4 + n].view(torch.int16) != out.view(torch.int16)).sum())
@@ -682,9 +568,8 @@ def check_temporal_conv_epilogue(b, f, h, w, c, cout, seed=0):
 def _epilogue_chain64(v, *, act=0, scale=1.0, rv=None, res=None, xs=None, alpha=None, multi=False):
     """The bf16 epilogue of the GEMM kernels applied in float64 to the pre-activation v (bias included): round, SiLU,
     scale, + row vector, + residual, AlphaBlender, rounding after each step.  -> (ref, rtol, mag).
-    Tolerance: one rounding: 1 ulp; bias + rounding + blend: check_linear_blend's 1 ulp of the largest intermediate; a row
-    vector and / or residual before it (or `multi`): 2 ulps of the largest intermediate (check_conv /
-    check_linear_rowvec)."""
+    Tolerance: one rounding: 1 ulp; bias + rounding + blend: 1 ulp of the largest intermediate; a row vector and / or
+    residual before it (or `multi`): 2 ulps of the largest intermediate, since two boundary flips can stack."""
     v = _r64(v)
     if act == 1:
         v = _r64(F.silu(v))
@@ -799,31 +684,40 @@ def linear_verdict(name, a, out, rerun, rows=None):
     return recs
 
 
-def conv2d_verdict(name, a, out, rerun, rows=None):
-    """ops.conv2d: the checks of linear_verdict on the channels-last output [N, Ho, Wo, Cout].  The float64 reference is
-    F.conv2d on the concatenated sources with the call's padding (pad (0, 1): one zero row / column at the bottom /
-    right).  rows: evaluate the reference on these images only (the kernel still runs on the whole launch)."""
-    x, x2, w, bias = a["x"], a["x2"], a["w_packed"], a["bias"]
+def conv2d_ref(a, rows=None, dtype=F64):
+    """The convolution of an ops.conv2d call (arguments `a`) in `dtype`: F.conv2d on the concatenated sources with the
+    call's padding (pad (0, 1): one zero row / column at the bottom / right), plus the bias when the call has one.
+    -> (out, sum |x_k w_k|), both channels-last [N, Ho, Wo, Cout].  rows: these images only."""
+    x, x2, w, bias = a["x"], a.get("x2"), a["w_packed"], a.get("bias")
     k, stride = a["ksize"], a["stride"]
-    if a["act"] == 2:
-        raise NotImplementedError("conv2d: GEGLU")
     ii = slice(None) if rows is None else torch.tensor(rows, device=x.device)
     xin = x[ii] if x2 is None else torch.cat([x[ii], x2[ii]], dim=3)
     ct, cout = xin.shape[3], w.shape[0]
-    kpt = a["k_per_tap"] if a["k_per_tap"] is not None else w.shape[1] // (k * k)
-    wt = w.to(F64).reshape(cout, k * k, kpt)[:, :, :ct].permute(0, 2, 1).reshape(cout, ct, k, k)
-    xd = xin.to(F64).permute(0, 3, 1, 2)
-    pad = (k // 2, k // 2) if a["pad"] is None else tuple(a["pad"])
+    kpt = a["k_per_tap"] if a.get("k_per_tap") is not None else w.shape[1] // (k * k)
+    wt = w.to(dtype).reshape(cout, k * k, kpt)[:, :, :ct].permute(0, 2, 1).reshape(cout, ct, k, k)
+    xd = xin.to(dtype).permute(0, 3, 1, 2)
+    pad = (k // 2, k // 2) if a.get("pad") is None else tuple(a["pad"])
     if pad == (0, 1):
         xd, padding = F.pad(xd, (0, 1, 0, 1)), 0
     else:
         padding = pad[0]
-    exact = F.conv2d(xd, wt, None if bias is None else bias.to(F64), stride=stride, padding=padding).permute(0, 2, 3, 1)
-    atol = _sum_floor(F.conv2d(xd.abs(), wt.abs(), stride=stride, padding=padding).permute(0, 2, 3, 1))
+
+    def conv(x_, w_, b_=None):
+        return F.conv2d(x_, w_, b_, stride=stride, padding=padding).permute(0, 2, 3, 1)
+    return conv(xd, wt, None if bias is None else bias.to(dtype)), conv(xd.abs(), wt.abs())
+
+
+def conv2d_verdict(name, a, out, rerun, rows=None):
+    """ops.conv2d: the checks of linear_verdict on the channels-last output [N, Ho, Wo, Cout] against conv2d_ref.
+    rows: evaluate the reference on these images only (the kernel still runs on the whole launch)."""
+    if a["act"] == 2:
+        raise NotImplementedError("conv2d: GEGLU")
+    exact, abs_sum = conv2d_ref(a, rows)
+    atol = _sum_floor(abs_sum)
+    del abs_sum
     # torch's own fp32 convolution on the same values: how far an fp32 accumulation of this launch lands from float64
-    fp32_err = float((F.conv2d(xd.float(), wt.float(), None if bias is None else bias.float(), stride=stride,
-                               padding=padding).permute(0, 2, 3, 1) - exact).abs().max())
-    del xd
+    fp32_err = float((conv2d_ref(a, rows, torch.float32)[0] - exact).abs().max())
+    ii = slice(None) if rows is None else torch.tensor(rows, device=out.device)
     dims = ("img", "y", "x", "ch")
     f64 = (lambda t: None if t is None else t[ii].to(F64))
     if a["out_fp32"] and (a["act"] != 0 or a["rowvec"] is not None or a["residual"] is not None):
@@ -858,23 +752,38 @@ def conv2d_verdict(name, a, out, rerun, rows=None):
     return recs
 
 
-def temporal_conv_verdict(name, a, out, frames=None):
-    """ops.temporal_conv (Conv3d (3, 1, 1) over the frames, zero frames at both ends of every clip): the float64 chain
-    with check_temporal_conv_epilogue's tolerance, 2 ulps of the largest intermediate (the op has no fp32 output).
-    frames: evaluate these output frames (of every clip) only."""
-    x, w, bias, f = a["x"], a["w_packed"], a["bias"], a["frames"]
+def temporal_conv_ref(a, frames=None):
+    """The float64 Conv3d (3, 1, 1) of an ops.temporal_conv call (arguments `a`) over the frames, zero frames at both
+    ends of every clip, plus the bias when the call has one.  -> (out, sum |x_k w_k|), both [clip, frame, pixel,
+    Cout].  frames: these output frames (of every clip) only."""
+    x, w, bias, f = a["x"], a["w_packed"], a.get("bias"), a["frames"]
     bf, h, w_, c = x.shape
     b, cout = bf // f, w.shape[0]
     fi = list(range(f)) if frames is None else list(frames)
     x4 = x.reshape(b, f, h * w_, c)
     wd = w.to(F64).reshape(cout, 3, w.shape[1] // 3)[:, :, :c]
     acc = torch.zeros(b, len(fi), h * w_, cout, dtype=F64, device=x.device)
+    abs_sum = torch.zeros_like(acc)
     for j, fr in enumerate(fi):
         for t in range(3):
             if 0 <= fr + t - 1 < f:
-                acc[:, j] += x4[:, fr + t - 1].to(F64) @ wd[:, t].t()
+                xt = x4[:, fr + t - 1].to(F64)
+                acc[:, j] += xt @ wd[:, t].t()
+                abs_sum[:, j] += xt.abs() @ wd[:, t].abs().t()
     if bias is not None:
         acc += bias.to(F64)
+    return acc, abs_sum
+
+
+def temporal_conv_verdict(name, a, out, frames=None):
+    """ops.temporal_conv (Conv3d (3, 1, 1) over the frames, zero frames at both ends of every clip): the float64 chain
+    with check_temporal_conv_epilogue's tolerance, 2 ulps of the largest intermediate (the op has no fp32 output).
+    frames: evaluate these output frames (of every clip) only."""
+    f = a["frames"]
+    bf, h, w_, _ = a["x"].shape
+    b, cout = bf // f, a["w_packed"].shape[0]
+    fi = list(range(f)) if frames is None else list(frames)
+    acc = temporal_conv_ref(a, fi)[0]
     rv = a["rowvec"]
     if rv is not None:
         rv = rv.to(F64).reshape(b, f, 1, cout)[:, fi] if rv.shape[0] > 1 else rv.to(F64).reshape(1, 1, 1, cout)
@@ -1263,42 +1172,7 @@ def run_all(stop_on_fail=False, group=None):
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
     RESULTS.clear()
-    groups = {"gemm": [
-        lambda: check_linear(256, 64, 64),
-        lambda: check_linear(128, 128, 128, bias=False),
-        lambda: check_linear(1000, 512, 320),
-        lambda: check_linear(4096, 320, 512, out_fp32=False),
-        lambda: check_linear(300, 2048, 1280, out_fp32=False, residual=True),
-        lambda: check_linear(77 * 2, 768, 320, bn=64),
-        lambda: check_linear(16, 320, 1280, out_fp32=False, act="silu"),
-        lambda: check_linear(50000, 512, 640, out_fp32=False, bn=128),
-        lambda: check_geglu(1024, 512, 2048),
-        lambda: check_linear_rowvec(1024, 512, 512, 256),
-        lambda: check_linear_rowvec(192, 320, 320, 64),
-        lambda: check_linear_blend(512, 2048, 512),
-        # lean epilogue specialisations (bias / bias+residual / GEGLU) over every BN and ragged edges
-        lambda: check_linear(3000, 640, 640, out_fp32=False, residual=True),       # BN 160: 80-column warp shares
-        lambda: check_linear(1100, 320, 1920, out_fp32=False),                      # BN 128, partial last M tile
-        lambda: check_linear(2048, 1280, 1280, out_fp32=False, residual=True),      # BN 256, two units per warp
-        lambda: check_linear(700, 256, 328, out_fp32=False, residual=True),         # n_out not a multiple of 64
-        lambda: check_linear(520, 192, 40, out_fp32=False, bias=False),             # BN 64, single partial unit
-        lambda: check_geglu(5000, 640, 2560),
-    ], "conv": [
-        lambda: check_conv(2, 16, 16, 64, 64),
-        lambda: check_conv(2, 32, 32, 320, 320),
-        lambda: check_conv(3, 8, 8, 1280, 1280, out_fp32=False, rowvec=True, residual=True),
-        lambda: check_conv(2, 64, 64, 320, 320, out_fp32=False, rowvec=True),
-        lambda: check_conv(2, 16, 16, 640, 320, ksize=1, out_fp32=False, residual=True),
-        lambda: check_conv(2, 16, 16, 640, 640, cin2=320, out_fp32=False),
-        lambda: check_conv(2, 32, 32, 320, 320, stride=2),
-        lambda: check_conv(2, 64, 64, 16, 32, stride=2),
-        lambda: check_conv(2, 64, 64, 8, 16),
-        lambda: check_conv(2, 24, 40, 96, 256, stride=2, out_fp32=False),
-        lambda: check_conv(2, 18, 32, 128, 64),
-        lambda: check_conv(2, 16, 16, 320, 320, ksize=1, out_fp32=False, scale=0.7),
-        lambda: check_temporal_conv(2, 16, 8, 8, 128, 128),
-        lambda: check_temporal_conv(1, 14, 16, 16, 320, 320),
-    ], "attn": [
+    groups = {"attn": [
         lambda: check_attention(1, 2, 256, 256, 64),
         lambda: check_attention(2, 5, 1024, 1024, 64),
         lambda: check_attention(2, 10, 1000, 77, 64),

@@ -448,17 +448,13 @@ def check_step_svd(steps=2, sparse=None):
 
 
 def check_extra_shapes():
-    """Kernel-level checks at shapes that first appear with the SVD / folded-conv / wide-tile work (576 x 1024 video ->
-    72 x 128 latents and its 36 x 64, 18 x 32 levels; K/V projection shape; folded conditioning convolutions)."""
+    """Attention checks at shapes that first appear with the SVD / wide-tile work (576 x 1024 video -> 72 x 128 latents
+    and its 36 x 64, 18 x 32 levels).  The GEMM calls at these levels are cases of tests/test_gemm_epilogue_exact_gpu.py."""
     from tests import kernel_checks as kc
     kc.RESULTS.clear()
     recs = [kc.check_attention(1, 5, 16384, 16384, 64),  # the dominant SDXL adapter-A shape (128^2 tokens), per sample
             kc.check_attention(1, 5, 2304, 2304, 64), kc.check_attention(2, 10, 576, 576, 64),
-            kc.check_attention(2, 20, 144, 144, 64), kc.check_temporal_attention(2, 14, 144, 10),
-            kc.check_conv(2, 36, 64, 320, 320, out_fp32=False, residual=True),
-            kc.check_conv(2, 18, 32, 640, 640, out_fp32=False, rowvec=True),
-            kc.check_conv(2, 64, 16, 64, 128, out_fp32=False), kc.check_conv(1, 64, 32, 64, 64, out_fp32=False),
-            kc.check_linear(1232, 2048, 2560, out_fp32=False), kc.check_linear(4608, 320, 960, out_fp32=False)]
+            kc.check_attention(2, 20, 144, 144, 64), kc.check_temporal_attention(2, 14, 144, 10)]
     for r in recs:
         RESULTS.append(r)
     return recs

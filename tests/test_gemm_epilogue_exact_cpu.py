@@ -4,7 +4,16 @@ The correct emulation (tests/ops_emulator.py, whose GEGLU honours the N tile, th
 as the kernel does) passes the exact check on every case below.  Each wrong variant of the epilogue chain -- the kind
 of change an epilogue rewrite makes by accident -- passes the float64 verdict that the layout checks and the launch
 census apply to the same call (kernel_checks.linear_verdict, launch_checks.VERIFIERS["linear"]) -- or, for GEGLU with
-a scale, gets no float64 verdict at all -- and fails the exact check.  An unrounded 1 - alpha is flagged by both.  `-s` prints `old verdicts: pass; exact: n differing at (r, c)` per variant."""
+a scale, gets no float64 verdict at all -- and fails the exact check.  An unrounded 1 - alpha is flagged by both.  `-s` prints `old verdicts: pass; exact: n differing at (r, c)` per variant.
+
+Two wrong variants that every instantiation shares -- a main loop that drops the last 64-wide K block, and an
+element-wise drain that also writes one column past its output slot -- pass the exact check, whose accumulators come
+from the same op layer, and fail the accumulator verdict against float64 or the guard bytes around the slot.  `-s`
+prints `current exact check: pass; new: <accumulator verdict | guard bytes> fails` for each, after the correct
+emulation passing all three on the same call."""
+import functools
+import types
+
 import pytest
 import torch
 import torch.nn.functional as F
@@ -36,8 +45,9 @@ def _g(seed):
 
 
 def _call(*, m=512, k=128, n=256, act=0, bias=True, bias_scale=1.0, wscale=1.0, scale=1.0, kind=0, rpv=32, bn=0,
-          alpha=0.3027, seed=0):
-    """a linear's arguments (ops.linear's parameter names); kind: 1 row vector, 2 residual, 4 blend source"""
+          alpha=0.3027, out_slot=False, seed=0):
+    """a linear's arguments (ops.linear's parameter names); kind: 1 row vector, 2 residual, 4 blend source; out_slot:
+    the output a gx.slot view"""
     g = _g(seed)
     rn = lambda *s, sc=1.0: (torch.randn(*s, generator=g) * sc).to(BF16)  # noqa: E731
     w_rows = 2 * n if act == 2 else n
@@ -50,12 +60,15 @@ def _call(*, m=512, k=128, n=256, act=0, bias=True, bias_scale=1.0, wscale=1.0, 
                 rowvec=rn(m // rpv, n) if kind & 1 else None, rows_per_vec=rpv if kind & 1 else 0,
                 blend_src=rn(m, n) if kind & 4 else None,
                 blend_alpha=torch.tensor([alpha]).to(BF16).float() if kind & 4 else None,
-                out_scale=scale, out=None, out_fp32=False, bn=bn)
+                out_scale=scale, out=gx.slot(torch.full((m, n), float("nan")).to(BF16)) if out_slot else None,
+                out_fp32=False, bn=bn)
 
 
-def _exact(call, out, tables):
-    acc, gate = gx.accumulators("linear", call, emu)
+def _exact(call, out, tables, ops=emu):
+    """the exact check of the call's output, the accumulators taken from ops.linear"""
     bn = gx.resolved_bn("linear", call)
+    raw = gx.accumulators("linear", call, ops)
+    acc, gate = gx.geglu_halves(raw, bn) if call["act"] == 2 else (raw, None)
     bias = call["bias"]
     if call["act"] == 2 and bias is not None:
         bias = gx.geglu_halves(bias, bn)
@@ -190,3 +203,55 @@ def test_exact_check_catches_wrong_variant(variant, tables):
     else:
         assert old_ok in (True, None), f"{variant}: the old verdicts already fail it ({note})"
     assert not exact_ok, f"{variant}: the exact check passes it"
+
+
+# ---- wrong main loops and drains that every instantiation shares, so the exact check, which takes its accumulators
+# from the same op layer, cannot see them: the accumulator verdict against float64 and the guard bytes around an
+# output slot do ----
+@functools.wraps(emu.linear, assigned=())  # gx.accumulators reads ops.linear's signature
+def _k_block_dropped(x, w, *args, **kw):
+    """the main loop stops one 64-wide K block short, in the fp32 and the bf16 output alike"""
+    x = x.clone()
+    x[:, -64:] = 0
+    return emu.linear(x, w, *args, **kw)
+
+
+@functools.wraps(emu.linear, assigned=())
+def _past_the_slot(*args, out=None, **kw):
+    """the element-wise drain (an output off 16-byte alignment) also writes the column after the output's last"""
+    y = emu.linear(*args, out=out, **kw)
+    if out is not None and out.data_ptr() % 16:
+        torch.as_strided(out, (out.shape[0], 1), out.stride(), out.storage_offset() + out.shape[1]).copy_(out[:, -1:])
+    return y
+
+
+SHARED = {
+    "main loop drops the last 64-wide K block": (_k_block_dropped, dict(kind=2)),
+    "element-wise drain writes one column past the slot": (_past_the_slot, dict(kind=2, out_slot=True)),
+}
+
+
+def _checks(fn, tables, **kw):
+    """(exact check ok, accumulator verdict ok, guard bytes ok) of fn on _call(**kw), the accumulators from fn"""
+    call = _call(**kw)
+    ops = types.SimpleNamespace(linear=fn)
+    out = ops.linear(**call)
+    exact_ok = _exact(call, out, tables, ops)[0]
+    acc_ok = gx.accumulator_verdict("linear", "linear", call, gx.accumulators("linear", call, ops))["ok"]
+    guard_ok = call["out"] is None or gx.guard_intact(call["out"])
+    return exact_ok, acc_ok, guard_ok
+
+
+@pytest.mark.parametrize("variant", list(SHARED))
+def test_new_checks_catch_shared_error(variant, tables):
+    fn, kw = SHARED[variant]
+    word = lambda ok: "pass" if ok else "FAIL"  # noqa: E731
+    ref = _checks(emu.linear, tables, **kw)
+    print(f"correct emulation ({variant} call): current exact check: {word(ref[0])}; "
+          f"accumulator verdict: {word(ref[1])}; guard bytes: {word(ref[2])}")
+    assert all(ref), f"correct emulation: {ref}"
+    exact_ok, acc_ok, guard_ok = _checks(fn, tables, **kw)
+    caught = [name for name, ok in (("accumulator verdict", acc_ok), ("guard bytes", guard_ok)) if not ok]
+    print(f"{variant}: current exact check: {word(exact_ok)}; new: {' and '.join(caught) or 'nothing'} fails")
+    assert exact_ok, f"{variant}: the current exact check already fails it"
+    assert caught, f"{variant}: neither the accumulator verdict nor the guard bytes fail it"
